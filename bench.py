@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — sentences/sec of top-1 analysis (BASELINE.json metric) on N B200s.
+"""bench.py — sentences/sec of top-1 analysis (BASELINE.json metric) on N H100s.
 
   --config 2 (default) : batch=8192 synthetic Korean sentences (web.txt length dist), Knlm model, top-1        [BASELINE.json configs[1]]
   --config 3           : batch=65536, CoNg model (int8 scorer on tensor-core tiles)                            [configs[2]]
@@ -12,7 +12,9 @@ One "step" = one pass of the hot path (lattice kernel + Viterbi kernel + emit + 
   --impl reference : the UNMODIFIED reference's CPU implementation (oracle/_ref/ref_bench, all host threads, >= 5 passes in ONE
            process, median) on a bounded sample of the same workload; also reports the 1-thread figure (tools/Evaluator.cpp:315-329).
 Launch: python bench.py --gpus N --steps K --warmup W   (N > 1: under torchrun, one rank per GPU; or --inproc: ONE process driving
-N GPUs through kiwi_b200_init_multi, the library's own ordered fan-out)."""
+N GPUs through kiwi_b200_init_multi, the library's own ordered fan-out).
+--dump-outputs DIR: after the timed steps, write what the last e2e step returned to its caller (token fields, token offsets, sentence
+           scores, status) as DIR/<name>.npy; inputs are seeded, so two builds can be compared output for output."""
 import argparse, json, math, os, subprocess, sys, tempfile, threading, time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -26,7 +28,7 @@ CONFIGS = {
     4: dict(model="knlm", batch=65536, typo="basic", typo_frac=0.3, rotate=1, steps=5, scaling="weak"),
     5: dict(model="cong", batch=1 << 20, typo=None, typo_frac=0.0, rotate=1, steps=3, scaling="strong"),
     # not a BASELINE.json config: the SkipBigram model type (SURVEY 8a row a13).  Its kernel inserts paths one at a time (viterbi.cu
-    # exactInsertRound): correct on hardware, but 11 passes over 2048 sentences did not finish in 600 s (round 2, GPU call L) - no measured line yet
+    # exactInsertRound): exact, but slow on path-heavy sentences - no measured line yet
     6: dict(model="sbg", batch=256, typo=None, typo_frac=0.0, rotate=1, steps=1, scaling="weak"),
 }
 BLOCK = 8192      # synthetic sentences are generated in seeded blocks of 8192 (block b: seed SEED + b)
@@ -55,11 +57,40 @@ def gen_sentences(cfg, first_block, n, seed_base):
     return out
 
 
+HBM_PEAK_GBS = 3350.0       # H100 SXM data sheet (HBM3), not a measured figure
+INT8_PEAK_TOPS = 1979.0     # H100 SXM data sheet, dense int8 at up to 700 W, not a measured figure
+DUMP_SENTENCES = 8192       # --dump-outputs: at most this many sentences (a fixed, seeded sample of larger batches)
+DUMP_MAX_BYTES = 64 << 20
+
+
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured"
-    return 6650.0, "fallback"
+        return json.load(open(p)).get("hbm_gbs", HBM_PEAK_GBS), "measured"
+    return HBM_PEAK_GBS, "fallback"
+
+
+def dump_outputs(out_dir, res):
+    """Writes a BatchResult as <name>.npy files: integer fields as float64 (exact), scores as float32.  Batches of more than
+    DUMP_SENTENCES sentences are sampled by a seeded choice that depends on the batch size only, so that the same sentences are
+    written by every build."""
+    import numpy as np
+    n = len(res.token_offsets) - 1
+    idx = np.arange(n) if n <= DUMP_SENTENCES else np.sort(np.random.RandomState(0).choice(n, DUMP_SENTENCES, replace=False))
+    off = res.token_offsets.astype(np.int64)
+    counts = off[idx + 1] - off[idx]
+    take = np.concatenate([np.arange(off[i], off[i + 1]) for i in idx]) if len(idx) else np.zeros(0, np.int64)
+    tok = res.tokens[take]
+    arrays = {"sentence_index": idx.astype(np.float64), "token_offsets": np.concatenate([[0], np.cumsum(counts)]).astype(np.float64),
+              "sentence_scores": res.scores[idx].astype(np.float32), "status": res.status[idx].astype(np.float64),
+              "morph_id": tok["morph_id"].astype(np.float64), "tag": tok["tag"].astype(np.float64), "position": tok["position"].astype(np.float64),
+              "length": tok["length"].astype(np.float64), "token_scores": tok["score"].astype(np.float32)}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_MAX_BYTES:
+        raise SystemExit("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_MAX_BYTES))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def host_cpus():
@@ -160,6 +191,7 @@ def main():
     ap.add_argument("--cpu-sample", type=int, default=8192)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (kernel experiments)")
     ap.add_argument("--inproc", action="store_true", help="one process, --gpus N devices behind ONE handle (kiwi_b200_init_multi) instead of torchrun ranks")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's results as DIR/<name>.npy")
     args = ap.parse_args()
     cfg = dict(CONFIGS[args.config])
     if args.batch: cfg["batch"] = args.batch
@@ -337,7 +369,7 @@ def main():
         "ms_per_step": dev_ms / steps, "higher_is_better": True, "scaling": cfg["scaling"], "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload,
-                   "l2": "per-step scratch working set (GBs) exceeds the 126 MB L2%s; the read-only model stays resident as in steady state" % (" and %d distinct input batches rotate" % R if R > 1 else ""),
+                   "l2": "per-step scratch working set (GBs) exceeds the 50 MB L2%s; the read-only model stays resident as in steady state" % (" and %d distinct input batches rotate" % R if R > 1 else ""),
                    "parallelism": ("one process, one handle over %d devices (kiwi_b200_init_multi): round-robin shards, one host thread per device, ordered merge" % ndev) if inproc else
                                   "dp%d (sentence sharding, one NCCL broadcast of the model image at init, no steady-state collectives)" % world,
                    "wall_ms_per_step": 1000.0 * wall / steps if steps else None,
@@ -348,7 +380,7 @@ def main():
         "clocks": sampler.summary(),
         "roofline": {"bound": "hbm", "kernel": kernel, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if achieved else None,
                      "traffic": prof.get("dram_bytes_per_launch"),
-                     "peak_kind": peak_kind + " (MEASURED_PEAKS.json hbm_gbs)" if peak_kind == "measured" else "fallback 6650",
+                     "peak_kind": peak_kind + " (MEASURED_PEAKS.json hbm_gbs)" if peak_kind == "measured" else "fallback: H100 SXM data sheet HBM3",
                      "algorithmic_bytes_per_sentence": vit_b, "lattice_kernel_bytes_per_sentence": lat_b, "counters": csrc,
                      "kernel_ms_per_step": vit_per_step_ms, "lattice_ms_per_step": ms_lat / steps if steps else None,
                      "kernel_share_of_step": ms_vit / dev_ms if dev_ms and not inproc else None,
@@ -361,10 +393,12 @@ def main():
     if cfg["model"] == "cong":
         # the int8 gather GEMMs of progressMatrix: 2 * sum(m * n * dim) integer ops per sentence (counted by the instrumented oracle)
         ops = 2.0 * c.get("cgMacs", 0) / max(1, c["sentences"])
-        line["roofline"]["tensor"] = {"bound": "tensor", "unit": "TOP/s", "achieved": ops * n_local / (vit_per_step_ms / 1000.0) / 1e12 if vit_per_step_ms else None, "peak": 4500.0,
-                                      "peak_kind": "nominal dense int8 (no measured int8 peak in MEASURED_PEAKS.json)", "int8_ops_per_sentence": ops,
+        line["roofline"]["tensor"] = {"bound": "tensor", "unit": "TOP/s", "achieved": ops * n_local / (vit_per_step_ms / 1000.0) / 1e12 if vit_per_step_ms else None, "peak": INT8_PEAK_TOPS,
+                                      "peak_kind": "H100 SXM data sheet dense int8 (not measured)", "int8_ops_per_sentence": ops,
                                       "note": "the gather GEMMs are a small part of viterbi_cong_kernel's time; the kernel as a whole is latency / L2 bound like the Knlm one"}
     print(json.dumps(line))
+    if args.dump_outputs and res is not None:
+        dump_outputs(args.dump_outputs, res)
     if dist: dist.destroy_process_group()
     return 0
 

@@ -1,4 +1,4 @@
-/* kiwi_b200 — C ABI of the B200-native replacement for Kiwi's lattice-analysis hot path.
+/* kiwi_b200 — C ABI of the GPU-native (sm_90a) replacement for Kiwi's lattice-analysis hot path.
  *
  * The entry points below are exactly the ones the reference's FFI for this path binds
  * (/root/reference/include/kiwi/capi.h, implementation src/capi/kiwi_c.cpp); each declaration cites the

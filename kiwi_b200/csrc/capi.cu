@@ -424,7 +424,7 @@ kiwi_h kiwi_b200_init_from_image(const void* bytes, uint64_t size)
 	try
 	{
 		int n = 0;
-		if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) throw std::runtime_error("kiwi_b200 needs a CUDA device (sm_100a); there is no CPU fallback");
+		if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) throw std::runtime_error("kiwi_b200 needs a CUDA device (sm_90a); there is no CPU fallback");
 		if (g_device >= 0 && cudaSetDevice(g_device) != cudaSuccess) throw std::runtime_error("cudaSetDevice failed");
 		auto* h = new kiwi_s;
 		h->engine.reset(new Engine(bytes, size));
@@ -438,7 +438,7 @@ kiwi_h kiwi_b200_init_multi(const void* bytes, uint64_t size, const int* devices
 	try
 	{
 		int n = 0;
-		if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) throw std::runtime_error("kiwi_b200 needs a CUDA device (sm_100a); there is no CPU fallback");
+		if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) throw std::runtime_error("kiwi_b200 needs a CUDA device (sm_90a); there is no CPU fallback");
 		if (n_devices < 1) throw std::invalid_argument("kiwi_b200_init_multi: n_devices < 1");
 		for (int i = 0; i < n_devices; ++i) if (devices[i] < 0 || devices[i] >= n) throw std::invalid_argument("kiwi_b200_init_multi: no such device");
 		auto h = std::unique_ptr<kiwi_s>(new kiwi_s);

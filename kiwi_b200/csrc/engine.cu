@@ -477,7 +477,7 @@ namespace kb
 	{
 		std::vector<uint32_t> failed = failedIn;
 		static const uint32_t pathMul[2] = { 8, 64 }, nodeMul[2] = { 4, 16 };
-		const size_t budget = (size_t)24 << 30;      // bytes of path pool per sub-pass
+		const size_t budget = (size_t)4 << 30;       // bytes of path pool per sub-pass (the retry arena stays allocated with its handle)
 		Slot& s = slot_[0];
 		for (int round = 0; round < 2 && !failed.empty(); ++round)
 		{
@@ -542,8 +542,11 @@ namespace kb
 	}
 
 	// Public entry: batches of any size.  The scratch arenas are sized per pass, so a large batch (65536 / 1 M sentences)
-	// is cut into passes of at most MAX_UNITS_PER_PASS normalised units / MAX_SENT_PER_PASS sentences.
-	static constexpr size_t MAX_UNITS_PER_PASS = 2u << 20, MAX_SENT_PER_PASS = 16384;
+	// is cut into passes of at most MAX_UNITS_PER_PASS normalised units / MAX_SENT_PER_PASS sentences.  A slot's arena costs about
+	// 7.3 KB per unit (128 48-byte paths, 12 nodes), so 1.5 Mi units are ~11 GB per slot: an 8192-sentence batch of web-shaped text
+	// (~1.3 M units) stays one pass, and two handles with both slots grown, their retry arenas and the device path of one of them fit
+	// the 80 GB of an H100.
+	static constexpr size_t MAX_UNITS_PER_PASS = 3u << 19, MAX_SENT_PER_PASS = 16384;
 	static size_t passSentLimit()
 	{
 		// KIWI_B200_PASS_SENT: sentences per pass (experiments with the overlap of small passes); default 16384

@@ -93,9 +93,8 @@ namespace KB_VIT_NS
 	// modes; with KB_STAGE_CAP > 512 the unbounded `top1` mode (> 512 incoming paths, insertion order, no bucket capacity)
 	// also goes through the pipeline up to that many incoming paths - these nodes dominate the heaviest sentences of a
 	// batch, and the kernel time is the time of its heaviest sentence.
-	// Measured (profiles/r1b_experiments.md): at 1536 the larger shared-memory footprint costs a resident block per SM and the
-	// kernel gets slower (134.7 k vs 161 k sentences/s), so the shipped default stays 512; the mode-2 pipeline is kept for a
-	// staging area outside shared memory.
+	// A larger capacity costs shared memory and with it resident blocks per SM, so the shipped default stays 512; the mode-2
+	// pipeline is kept for a staging area outside shared memory.
 #ifndef KB_CG_UCAP
 #define KB_CG_UCAP 32
 #endif
@@ -2744,8 +2743,8 @@ namespace KB_VIT_NS
 		}
 	};
 
-	// registers: the Knlm kernel is fastest at 4 resident blocks (128 registers, measured against 3 / 5 / 6); the CoNg kernel's
-	// larger per-warp state spills less at 3 blocks (profiles/r1b_experiments.md)
+	// registers: 4 resident blocks for the Knlm kernel (128 registers); the CoNg kernel's larger per-warp state spills less at 3 blocks.
+	// The Makefile overrides both per build.
 	#ifndef KB_VIT_MIN_BLOCKS
 #define KB_VIT_MIN_BLOCKS (KB_CONG ? 3 : 4)
 #endif
@@ -3051,7 +3050,7 @@ namespace KB_VIT_NS
 			int perSm = 0, sms = 0;
 			cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, KB_VIT_KERNEL, WARPS_PER_BLOCK * 32, smemBytes);
 			cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, devId);
-			resident = perSm > 0 && sms > 0 ? perSm * sms : 148;
+			resident = perSm > 0 && sms > 0 ? perSm * sms : 132;
 		}
 		if (vq.solo_warps == 0 || vq.solo_warps > WARPS_PER_BLOCK) vq.solo_blocks = 0;
 		// the solo blocks' missing warps are made up for by as many extra blocks only if they would still be resident: they are not, so the

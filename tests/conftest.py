@@ -6,7 +6,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu on a machine that has one")
 
 
 @pytest.fixture(scope="session")

@@ -122,7 +122,7 @@ def test_reference_c_api_single_and_multi(kiwi, oracle):
 
 
 def test_large_batch_is_split_into_passes(kiwi):
-    """40 000 sentences exceed one device pass (16 384 sentences / 2 Mi units): the engine cuts the batch and
+    """40 000 sentences exceed one device pass (16 384 sentences / 1.5 Mi units): the engine cuts the batch and
     the concatenated result must equal the per-pass results (batch-composition invariance at scale)."""
     from kiwi_b200.synth import synth_batch
     base = synth_batch(2000, 12345)

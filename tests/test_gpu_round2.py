@@ -1,9 +1,9 @@
-"""GPU (-m gpu), round 2: parity of the BENCH batches themselves against the UNMODIFIED reference (oracle/_ref/ref_bench token
-dumps, all sentences, not a sample of the restatement), the engine-ownership / multi-device / pass-pipelining paths, and the
-remaining reference C-ABI entry points (kiwi_analyze, kiwi_analyze_m, kiwi_res_word_position / kiwi_res_sent_position)."""
+"""GPU (-m gpu), round 2: parity of the BENCH batches themselves against the UNMODIFIED reference (tokens that oracle/_ref/ref_bench
+dumped for the whole batch, stored for a fixed sample of sentences in tests/golden/refbench_*.npz by tests/golden/make_refbench.py),
+the engine-ownership / multi-device / pass-pipelining paths, and the remaining reference C-ABI entry points (kiwi_analyze,
+kiwi_analyze_m, kiwi_res_word_position / kiwi_res_sent_position)."""
 import ctypes as C
 import os
-import struct
 import subprocess
 import tempfile
 import numpy as np
@@ -14,73 +14,56 @@ from tests.orc import IMAGE, CONG_IMAGE, TYPO_IMAGES
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_BENCH = os.path.join(ROOT, "oracle", "_ref", "ref_bench")
+GOLDEN = os.path.join(ROOT, "tests", "golden")
 RTOL = 1e-4
 
 
-def _reference_dump(model, texts, typo=None):
-    """tokens of every sentence from the unmodified reference (oracle/_ref/ref_bench travels with the repo; /root/reference is not needed)"""
-    if not os.path.exists(REF_BENCH):
-        pytest.skip("oracle/_ref/ref_bench missing: run __graft_entry__.build() where /root/reference exists")
-    with tempfile.NamedTemporaryFile("w", suffix=".txt", delete=False, encoding="utf-8") as f:
-        for t in texts: f.write(t + "\n")
-        src = f.name
-    dump = src + ".bin"
-    env = dict(os.environ, KIWI_ARCH_TYPE="avx2", KB_MODEL_TYPE=model, KB_DUMP=dump)
-    if typo: env["KB_TYPO"] = typo
-    try:
-        threads = max(1, len(os.sched_getaffinity(0)))
-        out = subprocess.run([REF_BENCH, os.path.join(ROOT, "oracle", "_ref", "models", model + "_small"), src, str(threads), "1"], capture_output=True, text=True, env=env, timeout=1800)
-        assert out.returncode == 0, out.stderr[-800:]
-        raw = open(dump, "rb").read()
-    finally:
-        for p in (src, dump):
-            if os.path.exists(p): os.unlink(p)
-    n, = struct.unpack_from("<I", raw, 0)
-    assert n == len(texts)
-    o = 4; counts = np.zeros(n, np.int64); scores = np.zeros(n, np.float32); rows = []
-    for i in range(n):
-        nt, sc = struct.unpack_from("<If", raw, o); o += 8
-        counts[i] = nt; scores[i] = sc
-        rows.append(np.frombuffer(raw, dtype=kiwi_b200.TOKEN_DTYPE, count=nt, offset=o)); o += 16 * nt
-    return counts, scores, rows
+def _reference_golden(name):
+    """(sentence indices, token counts, sentence scores, token rows) of the unmodified reference for one stored batch"""
+    z = np.load(os.path.join(GOLDEN, "refbench_%s.npz" % name))
+    counts = z["counts"].astype(np.int64)
+    off = np.concatenate([[0], np.cumsum(counts)])
+    toks = np.frombuffer(z["tokens"].tobytes(), dtype=kiwi_b200.TOKEN_DTYPE)
+    return z["index"].astype(np.int64), counts, z["scores"], [toks[off[i]:off[i + 1]] for i in range(len(counts))]
 
 
-def _compare_with_reference(res, counts, scores, rows, texts, what):
-    got_counts = np.diff(res.token_offsets.astype(np.int64))
+def _compare_with_reference(res, idx, counts, scores, rows, texts, what):
+    got_counts = np.diff(res.token_offsets.astype(np.int64))[idx]
     bad = np.nonzero(got_counts != counts)[0]
-    assert len(bad) == 0, (what, "token counts differ", int(bad[0]), texts[int(bad[0])])
+    assert len(bad) == 0, (what, "token counts differ", int(idx[bad[0]]), texts[int(idx[bad[0]])])
     ref = np.concatenate(rows) if rows else np.zeros(0, kiwi_b200.TOKEN_DTYPE)
-    got = res.tokens
+    got = np.concatenate([res.sentence(int(i)) for i in idx]) if len(idx) else np.zeros(0, kiwi_b200.TOKEN_DTYPE)
+    off = np.concatenate([[0], np.cumsum(counts)])
     for f in ("morph_id", "position", "length", "tag"):
         d = np.nonzero(got[f] != ref[f])[0]
         if len(d):
-            s = int(np.searchsorted(res.token_offsets, d[0], side="right") - 1)
+            s = int(idx[np.searchsorted(off, d[0], side="right") - 1])
             raise AssertionError((what, f, "differs in sentence", s, texts[s]))
     tol = RTOL * np.maximum(1.0, np.abs(ref["score"]))
     assert (np.abs(got["score"] - ref["score"]) <= tol).all(), what
-    assert (np.abs(res.scores - scores) <= RTOL * np.maximum(1.0, np.abs(scores))).all(), what
-    exact = float((res.scores == scores).mean())
-    print("%s: %d sentences, %d tokens identical to the unmodified reference; %.2f %% of the sentence scores bit-exact" % (what, len(texts), len(ref), 100 * exact))
+    got_scores = res.scores[idx]
+    assert (np.abs(got_scores - scores) <= RTOL * np.maximum(1.0, np.abs(scores))).all(), what
+    exact = float((got_scores == scores).mean())
+    print("%s: %d sampled sentences, %d tokens identical to the unmodified reference; %.2f %% of the sentence scores bit-exact" % (what, len(idx), len(ref), 100 * exact))
     assert exact >= 0.99
 
 
 def test_bench_batch_config2_all_sentences_match_reference(kiwi):
-    """every sentence of the config-2 bench batch (8192, Knlm) against the reference's own tokens"""
+    """the config-2 bench batch (8192, Knlm) against the reference's own tokens (stored sample)"""
     import bench
     from kiwi_b200.synth import SEED
     texts = bench.gen_sentences(bench.CONFIGS[2], 0, 8192, SEED)
     res = kiwi.analyze_batch(texts)
-    _compare_with_reference(res, *_reference_dump("knlm", texts), texts, "config 2")
+    _compare_with_reference(res, *_reference_golden("cfg2"), texts, "config 2")
 
 
 def test_bench_batch_config3_cong_65536_matches_reference(kiwi_cong):
-    """config 3 at its stated size: 65536 sentences, CoNg model, all sentences against the reference (multi-pass engine path)"""
+    """config 3 at its stated size: 65536 sentences, CoNg model, against the reference (stored sample; multi-pass engine path)"""
     import bench
     from kiwi_b200.synth import SEED
     texts = bench.gen_sentences(bench.CONFIGS[3], 0, 65536, SEED)
     res = kiwi_cong.analyze_batch(texts)
-    _compare_with_reference(res, *_reference_dump("cong", texts), texts, "config 3")
+    _compare_with_reference(res, *_reference_golden("cfg3"), texts, "config 3")
 
 
 def test_bench_batch_config4_typo_65536_matches_reference(kiwi):
@@ -92,7 +75,7 @@ def test_bench_batch_config4_typo_65536_matches_reference(kiwi):
     texts = bench.gen_sentences(cfg, 0, 65536, SEED)
     typo = kiwi_b200.PreparedTypo(path=TYPO_IMAGES["basic"])
     res = kiwi.analyze_batch(texts, kiwi_b200.default_option(typo=typo))
-    _compare_with_reference(res, *_reference_dump("knlm", texts, typo="basic"), texts, "config 4")
+    _compare_with_reference(res, *_reference_golden("cfg4"), texts, "config 4")
     plain = kiwi.analyze_batch(texts[:4096])
     changed = sum(1 for i in range(4096) if plain.sentence(i).tobytes() != res.sentence(i).tobytes())
     print("config 4: the typo lattice changes %d of the first 4096 analyses" % changed)
@@ -228,9 +211,11 @@ def test_top1_container_and_full_bucket_cases_match_reference(kiwi, oracle):
         prev = c
     print("%d of %d bench sentences use the top1 container or hit a full bucket" % (len(hard), len(texts)))
     assert len(hard) >= 8
+    idx, counts, scores, rows = _reference_golden("top1")
+    assert hard == idx.tolist()
     sub = [texts[i] for i in hard]
     res = kiwi.analyze_batch(sub)
-    _compare_with_reference(res, *_reference_dump("knlm", sub), sub, "top1 / full-bucket sentences")
+    _compare_with_reference(res, np.arange(len(sub)), counts, scores, rows, sub, "top1 / full-bucket sentences")
 
 
 def test_input_text_never_fails_the_batch(kiwi, oracle):

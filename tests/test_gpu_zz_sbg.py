@@ -23,10 +23,9 @@ def kiwi_sbg():
     kw.close()
 
 
-# Measured on a B200 (round 2, GPU call L): all 33 + 158 sentences of inputs_written / inputs_web pass, bit for bit.  The SkipBigram
-# kernel inserts paths one at a time and is slow on inputs whose path sets explode (the first 300 of inputs_ref_tests did not finish in
-# 13 minutes; the reference itself needs minutes and tens of GB on the later ones), so the suite keeps to the two corpus files, and this
-# file sorts last among the GPU tests.
+# The SkipBigram kernel inserts paths one at a time and is slow on inputs whose path sets explode (the reference itself needs minutes
+# and tens of GB on the later sentences of inputs_ref_tests), so the suite keeps to the two corpus files, and this file sorts last among
+# the GPU tests.
 @pytest.mark.timeout(1200)
 @pytest.mark.parametrize("name,limit", [("inputs_written", None), ("inputs_web", 80)])
 def test_sbg_tokens_and_scores_match_reference_golden(kiwi_sbg, name, limit):

@@ -2,19 +2,19 @@
 kiwi_b200_native_sbg / kiwi_b200_native_cong; SURVEY 8f-2, first pieces of a loader that does not link the reference).  tests/native/native_lm_check.cpp
 compares their output with the Knlm / SkipBigram / CoNg sections of the model images that flatten_model dumped from the reference's own
 in-memory models: every section byte for byte, and the scalars the reference computes at load time (suffix links, BOS state, unk_ll)."""
-import os, subprocess, tempfile
+import os, subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODELS = os.path.join(ROOT, "oracle", "_ref", "models")
 
 
-def test_native_knlm_and_sbg_sections_equal_the_flattened_image():
+def test_native_knlm_and_sbg_sections_equal_the_flattened_image(tmp_path):
     lib = os.path.join(ROOT, "kiwi_b200", "libkiwi_b200.so")
     knlm_img = os.path.join(MODELS, "knlm_small.img"); knlm_file = os.path.join(MODELS, "knlm_small", "sj.knlm")
     if not (os.path.exists(lib) and os.path.exists(knlm_img) and os.path.exists(knlm_file)):
         pytest.skip("library, model image or the reference-format model directory missing: run __graft_entry__.build()")
-    exe = os.path.join(tempfile.gettempdir(), "kb_native_lm_check")
+    exe = str(tmp_path / "kb_native_lm_check")
     subprocess.run(["g++", "-O2", "-std=c++17", "-o", exe, os.path.join(ROOT, "tests", "native", "native_lm_check.cpp"), "-ldl"], check=True)
     args = [exe, lib, knlm_img, knlm_file]
     sbg_img = os.path.join(MODELS, "sbg_small.img"); sbg_file = os.path.join(MODELS, "sbg_small", "skipbigram.mdl")
