@@ -22,6 +22,9 @@
 // 4 x 128 "medium" mode).  Pruning is a warp max-reduction followed by a ballot compaction.
 // Compile with -fmad=false: the reference's float sums are not contracted (x86-64 baseline, no FMA).
 #include <cstdlib>
+#ifdef KB_HOSTSIM
+#include <unordered_set>
+#endif
 #include <cuda_runtime.h>
 #include <math_constants.h>
 #include "kb_model.h"
@@ -93,7 +96,8 @@ namespace KB_VIT_NS
 	// modes; with KB_STAGE_CAP > 512 the unbounded `top1` mode (> 512 incoming paths, insertion order, no bucket capacity)
 	// also goes through the pipeline up to that many incoming paths - these nodes dominate the heaviest sentences of a
 	// batch, and the kernel time is the time of its heaviest sentence.
-	// A larger capacity costs shared memory and with it resident blocks per SM, so the shipped default stays 512; the mode-2
+	// A larger capacity costs shared memory (one byte per path and warp), and the L1 cache shrinks with every step of the shared-memory
+	// carveout: the Knlm build (one block of 12 warps per SM) stages 1024 paths (csrc/Makefile), the other builds 512.  The mode-2
 	// pipeline is kept for a staging area outside shared memory.
 #ifndef KB_CG_UCAP
 #define KB_CG_UCAP 32
@@ -295,8 +299,21 @@ namespace KB_VIT_NS
 			return KnRes{ acc + asFloat(v), nodeIdx };
 		}
 	}
+#if defined(KB_HOSTSIM) && !KB_CONG && !KB_SBG
+	// tests/hostsim: LM steps and distinct (state, wid) pairs of one sentence (scripts/lm_repeat.py reads and resets them per sentence)
+	static uint64_t g_lmSteps, g_lmDistinct;
+	static std::unordered_set<uint64_t> g_lmPairs;
+	extern "C" void hs32_lm_repeat_stats(uint64_t* out)
+	{
+		out[0] = g_lmSteps; out[1] = g_lmDistinct;
+		g_lmSteps = g_lmDistinct = 0; g_lmPairs.clear();
+	}
+#endif
 	__device__ __forceinline__ float knProgress(int32_t& nodeIdx, uint32_t next, uint32_t = 0)
 	{
+#if defined(KB_HOSTSIM) && !KB_CONG && !KB_SBG
+		++g_lmSteps; g_lmDistinct += g_lmPairs.insert((uint64_t)(uint32_t)nodeIdx << 32 | next).second;
+#endif
 		const KnRes r = knProgressV(nodeIdx, next);
 		nodeIdx = r.node;
 		return r.ll;
