@@ -520,10 +520,12 @@ namespace KB_VIT_NS
 #else
 #define KB_INL_EVAL __noinline__
 #endif
+	// Vit lives in local memory (its address is `this` of the out-of-line members), and every member a loop reads through `this` is
+	// re-read from there after each store the compiler cannot tell apart from it.  The hot loops (flushItems, evaluate) therefore work
+	// on register copies of the members they read.  The kernel parameters are not referenced from here: a reference would give them
+	// a local copy too.
 	struct Vit
 	{
-		const BatchView& bv;
-		const VitView& vv;
 		const uint32_t lane;
 		uint32_t err = 0;
 		// sentence
@@ -540,7 +542,7 @@ namespace KB_VIT_NS
 #endif
 		DCand* dcur = nullptr; uint32_t curBuf = 0, pfPhase = 0; const DCand* pfBase[2] = { nullptr, nullptr };      // candidate-row staging (see prefetchCands)
 		uint2* nodeCand = nullptr;
-		WarpSmem* sm; uint32_t stagedNode = 0xFFFFFFFFu; uint32_t nItems = 0; uint32_t htBase = 0, htCount = 0, nFw = 1;
+		WarpSmem* sm; uint32_t stagedNode = 0xFFFFFFFFu; uint32_t htBase = 0, htCount = 0;
 		uint32_t nClasses = 0, classCommon = 0; bool classOverflow = false;
 		// team mode (the heaviest sentences): KB_TEAM warps share one sentence, see TeamSmem
 #if KB_TEAM > 1
@@ -550,7 +552,7 @@ namespace KB_VIT_NS
 #endif
 		bool splitComplex, splitSaisiot, mergeSaisiot;
 
-		__device__ Vit(const BatchView& _bv, const VitView& _vv, uint32_t _lane) : bv{ _bv }, vv{ _vv }, lane{ _lane } {}
+		__device__ explicit Vit(uint32_t _lane) : lane{ _lane } {}
 
 		// ---- team primitives (no-ops for a single warp)
 		__device__ __forceinline__ bool leader() const { return teamRank == 0; }
@@ -1245,7 +1247,7 @@ namespace KB_VIT_NS
 						if (accepted)
 						{
 							uint32_t slot = htHash(lmState, prevRoot, spState);
-							while (atomicCAS_u16(slot, newIdx + 1)) slot = (slot + 1) & (HT_SIZE - 1);
+							while (atomicCAS_u16(ht, slot, newIdx + 1)) slot = (slot + 1) & (HT_SIZE - 1);
 						}
 						E += totalNew;
 						htUsed = 1;
@@ -1258,7 +1260,7 @@ namespace KB_VIT_NS
 						if (isNew)
 						{
 							uint32_t slot = htHash(lmState, prevRoot, spState);
-							while (atomicCAS_u16(slot, newIdx + 1)) slot = (slot + 1) & (HT_SIZE - 1);
+							while (atomicCAS_u16(ht, slot, newIdx + 1)) slot = (slot + 1) & (HT_SIZE - 1);
 						}
 						E += totalNew;
 						htUsed = 1;
@@ -1331,7 +1333,7 @@ namespace KB_VIT_NS
 			top = candBeg + E;      // (mode 2: the container's write-out order is applied per candidate segment by fixupGroup)
 		}
 
-		__device__ __forceinline__ bool atomicCAS_u16(uint32_t slot, uint32_t val)
+		static __device__ __forceinline__ bool atomicCAS_u16(uint16_t* ht, uint32_t slot, uint32_t val)
 		{
 			// returns true when the slot was occupied (caller probes on).  16-bit CAS on a 32-bit word.
 			uint32_t* w = reinterpret_cast<uint32_t*>(ht) + (slot >> 1);
@@ -1449,9 +1451,17 @@ namespace KB_VIT_NS
 #endif
 		};
 
-		__device__ __noinline__ void flushItems(const FlushCtx& fc)
+		// the `nItems` items in sm->item; false when the pool overflowed (err is set).  Out of line: it has several call sites, and
+		// instruction-cache misses are the kernel's other large stall.  The members it reads are copied to registers (see Vit), and
+		// htCount / htUsed / top are written back once.
+		__device__ __noinline__ bool flushItems(const FlushCtx& fcIn, uint32_t nItems)
 		{
-			if (!nItems) return;
+			if (!nItems) return true;
+			const FlushCtx fc = fcIn;
+			PathT* const pool = this->pool; WarpSmem* const sm = this->sm; uint16_t* const ht = this->ht; const DCand* const dcur = this->dcur;
+			const uint32_t lane = this->lane, poolCap = this->poolCap, htBase = this->htBase;
+			const uint8_t uniq0 = uniq[0], uniq1 = uniq[1];
+			uint32_t htCount = this->htCount, htUsed = this->htUsed;
 			__syncwarp();
 			#pragma unroll 1
 			for (uint32_t ib = 0; ib < nItems; ib += 32)
@@ -1475,7 +1485,7 @@ namespace KB_VIT_NS
 					const uint32_t meta = *reinterpret_cast<const uint32_t*>(&pp->sp_state);   // sp_state | root_id << 8 | prev_root_id << 16 | morph_tag << 24
 					prevRoot = (meta >> 8) & 0xFF;
 					const bool doFork = (cd.flags & CS_FORK) && prevRoot == COMMON_ROOT;
-					spState = doFork ? uniq[r] : (uint8_t)(meta & 0xFF);
+					spState = doFork ? (r ? uniq1 : uniq0) : (uint8_t)(meta & 0xFF);
 					rootId = doFork ? (uint8_t)r : COMMON_ROOT;
 					typoAcc = __uint_as_float(s0.z);
 					float candScore = __uint_as_float(s0.y) + cd.additionalScore;
@@ -1594,11 +1604,15 @@ namespace KB_VIT_NS
 				const uint32_t totalNew = __popc(nmask);
 				uint32_t newIdx = NPOS;
 				if (isNew) newIdx = htCount + __popc(nmask & ((1u << lane) - 1));
-				if (htBase + htCount + totalNew > poolCap || htCount + totalNew > HT_MAX_ENTRIES) { err = ST_PATH_OVERFLOW; return; }
+				if (htBase + htCount + totalNew > poolCap || htCount + totalNew > HT_MAX_ENTRIES)
+				{
+					err = ST_PATH_OVERFLOW; this->htCount = htCount; this->htUsed = htUsed;
+					return false;
+				}
 				if (isNew)
 				{
 					uint32_t hs = h0;
-					while (atomicCAS_u16(hs, newIdx + 1)) hs = (hs + 1) & (HT_SIZE - 1);
+					while (atomicCAS_u16(ht, hs, newIdx + 1)) hs = (hs + 1) & (HT_SIZE - 1);
 					atomicAdd(&sm->candNew[slot], 1u);
 				}
 				if (totalNew) htUsed = 1;
@@ -1633,8 +1647,9 @@ namespace KB_VIT_NS
 				}
 				__syncwarp();
 			}
+			this->htCount = htCount; this->htUsed = htUsed;
 			top = htBase + htCount;
-			nItems = 0;
+			return true;
 		}
 
 		__device__ void resetIndex()
@@ -2016,6 +2031,8 @@ namespace KB_VIT_NS
 		__device__ KB_INL_EVAL void evaluate(uint32_t nodeIdx, uint32_t nodeBeg, const DCand* candBase, uint32_t nCandsIn,
 			float unkFormDiscount, uint32_t ownOff, uint32_t ownLen, uint32_t inBeg, uint32_t inEnd, bool first)
 		{
+			// register copies (see Vit)
+			WarpSmem* const sm = this->sm; PathT* const pool = this->pool; const uint32_t lane = this->lane, nUniq = this->nUniq;
 			// `first`: the node's first evaluation - its candidate block may be waiting in the other staging buffer
 			bool rowsStaged = false;
 #if KB_TMA_ROWS
@@ -2054,8 +2071,11 @@ namespace KB_VIT_NS
 			fc.inEnd = inEnd; fc.mode = mode; fc.spaceBefore = spaceBefore ? 1u : 0u;
 			if (itemOK) stagePaths(nodeIdx, inBeg, P);
 			const bool itemOK2 = itemOK && !classOverflow;
+			const uint32_t nClasses = this->nClasses, classCommon = this->classCommon;
 			if (ownLen) { uint16_t ol; uint8_t op; leftFeat(ownOff, ownLen, 0, 0, ol, op); fc.ownFw = fwOfLeft(ol, op); }
-			nItems = 0;
+			uint32_t nItems = 0;      // items waiting in sm->item
+			uint32_t nFw = 1;         // entries of sm->fwTab (index 0 unused)
+			auto flush = [&]() { const bool ok = flushItems(fc, nItems); nItems = 0; return ok; };
 			const bool snPoint = node.uform_len && norm[node.uform_off + node.uform_len - 1] == '.';
 			const uint32_t nWords = (P + 31) >> 5;
 			// class of lane's path in each of the first 6 words of 32 incoming paths, 5 bits each (+ which words have a path for this lane): the
@@ -2223,7 +2243,7 @@ namespace KB_VIT_NS
 							if (!(vmK | setsK)) continue;
 							const uint32_t cfK = __shfl_sync(FULL, myCondFail, k);
 							// the entry index is shared by consecutive candidates while it is small; a top1-mode candidate (up to P entries) starts with an empty one
-							if (mode == 2 ? (htCount | nItems) != 0 : htCount + nItems > 256) { flushItems(fc); if (err) return; resetIndex(); }
+							if (mode == 2 ? (htCount | nItems) != 0 : htCount + nItems > 256) { if (!flush()) return; resetIndex(); }
 							if (!(kfl & CS_FORK) && !setsK)
 							{
 								// common case: the survivors of every 32 incoming paths are compacted by one ballot, in path order
@@ -2237,7 +2257,7 @@ namespace KB_VIT_NS
 									const unsigned m = __ballot_sync(FULL, on);
 									if (!m) continue;
 									const uint32_t cnt = __popc(m);
-									if (nItems + cnt > ITEM_CAP) { flushItems(fc); if (err) return; }
+									if (nItems + cnt > ITEM_CAP) { if (!flush()) return; }
 									if (on) sm->item[nItems + __popc(m & ((1u << lane) - 1))] = (k << 27) | (q << 3) | ((cfK >> c) & 1u);
 									nItems += cnt;
 								}
@@ -2254,7 +2274,7 @@ namespace KB_VIT_NS
 							#pragma unroll 1
 							for (uint32_t qb = 0; qb < P; qb += perRound)
 							{
-								if (nItems + 32 > ITEM_CAP) { flushItems(fc); if (err) return; }
+								if (nItems + 32 > ITEM_CAP) { if (!flush()) return; }
 								const uint32_t pr = lane >> rshift, rr = lane & ((1u << rshift) - 1);
 								const uint32_t q = qb + pr;
 								bool valid = false, condFail = false, setsFW = false, isSock = false;
@@ -2311,7 +2331,7 @@ namespace KB_VIT_NS
 							continue;
 						}
 						// general path and shortcuts: drain the pipeline first so that entries stay candidate-major
-						flushItems(fc); if (err) return;
+						if (!flush()) return;
 						const uint32_t before = top;
 						GenCtx g;
 						g.nodeIdx = nodeIdx; g.inBeg = inBeg; g.inEnd = inEnd; g.mode = mode; g.ownOff = ownOff; g.ownLen = ownLen; g.ownFw = fc.ownFw;
@@ -2325,7 +2345,7 @@ namespace KB_VIT_NS
 						__syncwarp();
 						resetIndex();
 					}
-					flushItems(fc); if (err) return;
+					if (!flush()) return;
 #if !KB_SBG && !defined(KB_NO_EXACT_REDO)
 					// The parallel insert above is the reference's container as long as no bucket reaches 64 states (0.02 % of the containers
 					// of the bench batches do).  Beyond that the reference's insertOptimized behaves differently (exactInsertRound): the
@@ -2795,7 +2815,7 @@ namespace KB_VIT_NS
 		bool firstDraw = true;
 		uint32_t pfPhaseKeep = 0, curBufKeep = 0;
 #if KB_TMA_ROWS
-		{ Vit v0{ bv, vv, lane }; v0.sm = &smAll[wib]; v0.pfInit(); }
+		{ Vit v0{ lane }; v0.sm = &smAll[wib]; v0.pfInit(); }
 #endif
 		for (;;)
 		{
@@ -2833,7 +2853,7 @@ namespace KB_VIT_NS
 		const size_t nbase = (size_t)bv.nodes_per_unit * wbase;
 		const size_t pbase = (size_t)vv.paths_per_unit * wbase + (size_t)vv.paths_const * s;
 
-		Vit v{ bv, vv, lane };
+		Vit v{ lane };
 		v.norm = bv.norm + wbase;
 		v.pool = reinterpret_cast<PathT*>(vv.paths) + pbase;      // (records of VitView::path_stride bytes)
 		v.poolCap = vv.paths_per_unit * W + vv.paths_const;
