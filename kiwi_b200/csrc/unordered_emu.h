@@ -8,7 +8,8 @@
 // set is cleared, never shrunk, between uses - and (b) the hash codes of the distinct keys in first-insertion order; the kernels know
 // both: keys are appended in first-insertion order, and the bucket count is a per-sentence state that starts at 1 like the oracle's
 // (the reference's thread_local set additionally remembers earlier sentences of its thread: not reproducible by definition).
-// Sequential (one lane); n = distinct keys of one candidate's container (hundreds).
+// unorderedSetOrder is the sequential statement; the kernels run unorderedSetOrderWarp, the same order computed by a whole warp.
+// n = distinct keys of one candidate's container (hundreds).
 #pragma once
 #include <stdint.h>
 
@@ -95,4 +96,84 @@ namespace kb
 		bucketCount = B;
 		return j == n;
 	}
+
+#if defined(__CUDACC__) || defined(KB_HOSTSIM)
+	// The same order computed by a whole warp; unorderedSetOrder above is its specification.  Every lane calls it with the same arguments.
+	//
+	// _M_insert_bucket_begin and the relink loop of _M_rehash_aux apply one rule: a node whose bucket already holds nodes goes to the
+	// front of that bucket's run, any other node to the head of the list.  So within an epoch (a stretch with one bucket count B), whose
+	// ARRIVALS are the list left by the rehash followed by the epoch's insertions, the list is: buckets by descending arrival of their
+	// first node, and within a bucket, nodes by descending arrival.  Per epoch: (1) bucket and first arrival of every node, 32 arrivals
+	// a round, node count per bucket kept at the bucket's first arrival; (2) suffix sum of those counts over the arrivals = where each
+	// bucket's run starts; (3) scatter, arrivals in descending order, each bucket's run filled from its start.
+	//
+	// codeOf(i): hash code of the i-th distinct key in first-insertion order.  bucketCount: in = the set's bucket count before the first
+	// insertion, out = after the last.  first[n], runs[n], buckets[bucketCount after]: scratch.  order[n] as in unorderedSetOrder.
+	// Returns false when the bucket chain is exhausted.
+	template<class CodeOf>
+	__device__ inline bool unorderedSetOrderWarp(CodeOf codeOf, int32_t n, uint32_t& bucketCount, int32_t* first, int32_t* runs, int32_t* buckets, int32_t* order, uint32_t lane)
+	{
+		const unsigned FULL = 0xFFFFFFFFu;
+		uint32_t B = bucketCount;
+		int32_t m = 0;      // nodes in the list; order[0, m) is the list
+		while (m < n)
+		{
+			if ((uint32_t)m + 1 > (B == 1 ? 0u : B)) { B = unorderedNextBuckets(B); if (!B) return false; }
+			const int32_t m1 = (int32_t)B < n ? (int32_t)B : n;      // insertions m .. m1 - 1 keep this bucket count
+			for (uint32_t b = lane; b < B; b += 32) buckets[b] = -1;
+			for (int32_t t = (int32_t)lane; t < m1; t += 32) runs[t] = 0;
+			__syncwarp();
+			// (1) arrival t is node order[t] (t < m: the relinked list) or node t (this epoch's insertions)
+			for (int32_t base = 0; base < m1; base += 32)
+			{
+				const int32_t t = base + (int32_t)lane;
+				const bool valid = t < m1;
+				const uint32_t bkt = valid ? (uint32_t)(codeOf(t < m ? order[t] : t) % B) : 0xFFFFFFFFu;
+				const unsigned grp = __match_any_sync(FULL, bkt);
+				const int32_t leader = __ffs(grp) - 1;
+				int32_t f = 0;
+				if (valid && (int32_t)lane == leader)
+				{
+					f = buckets[bkt];
+					if (f < 0) { f = t; buckets[bkt] = t; }
+					runs[f] += __popc(grp);
+				}
+				f = __shfl_sync(FULL, f, leader);
+				if (valid) first[t] = f;
+				__syncwarp();
+			}
+			// (2) runs[t] = nodes of the buckets whose first arrival is after t = start of the run of the bucket first reached at t
+			int32_t carry = 0;
+			for (int32_t base = (m1 - 1) & ~31; base >= 0; base -= 32)
+			{
+				const int32_t t = base + (int32_t)lane;
+				const int32_t c = t < m1 ? runs[t] : 0;
+				int32_t incl = c;      // inclusive suffix sum inside the round
+				for (int d = 1; d < 32; d <<= 1) { const int32_t o = __shfl_down_sync(FULL, incl, d); if (lane + d < 32) incl += o; }
+				if (t < m1) runs[t] = carry + incl - c;
+				carry += __shfl_sync(FULL, incl, 0);
+			}
+			__syncwarp();
+			// (3) the bucket array is dead: it receives the new list.  Later arrivals of a bucket come first.
+			for (int32_t base = (m1 - 1) & ~31; base >= 0; base -= 32)
+			{
+				const int32_t t = base + (int32_t)lane;
+				const bool valid = t < m1;
+				const int32_t f = valid ? first[t] : -1;
+				const unsigned grp = __match_any_sync(FULL, f);
+				const int32_t leader = __ffs(grp) - 1;
+				int32_t at = 0;
+				if (valid && (int32_t)lane == leader) { at = runs[f]; runs[f] = at + __popc(grp); }
+				at = __shfl_sync(FULL, at, leader);
+				if (valid) buckets[at + __popc(grp & ~((2u << lane) - 1u))] = t < m ? order[t] : t;
+				__syncwarp();
+			}
+			for (int32_t t = (int32_t)lane; t < m1; t += 32) order[t] = buckets[t];
+			__syncwarp();
+			m = m1;
+		}
+		bucketCount = B;
+		return true;
+	}
+#endif
 }

@@ -79,6 +79,23 @@ namespace KB_VIT_NS
 	// the model view lives in constant memory: every `c_m.field` is an immediate-offset constant-bank load
 	__constant__ DevModel c_m;
 
+#if KB_PHASE_CLOCKS
+	// Diagnostic build only (`make variant VFLAGS="... -DKB_PHASE_CLOCKS"`, scripts/phase_clocks.py): clock64 cycles of the phases of
+	// each sentence's Viterbi, summed over the sentence, lane 0 of its warp, and what its `top1` containers held (count, entries, bucket
+	// count after each, rehashes); sentences with index >= KB_PHASE_SENT are not counted
+	enum { PH_TOP1_ORDER, PH_TOP1_REORDER, PH_FLUSH, PH_EVALUATE, PH_PRUNE, PH_NODE_LOOP, PH_FIND_BEST_PATH,
+	       PH_N_TOP1, PH_SUM_E, PH_SUM_B, PH_REHASHES, PH_COUNT };
+	constexpr uint32_t KB_PHASE_SENT = 8192;
+	__device__ unsigned long long phaseClocks[KB_PHASE_SENT * PH_COUNT];
+#define KB_PH_START(t) const long long t = clock64()
+#define KB_PH_ADD(ph, t, sent) do { if (lane == 0 && (sent) < KB_PHASE_SENT) phaseClocks[(sent) * PH_COUNT + (ph)] += (unsigned long long)(clock64() - (t)); } while (0)
+#define KB_PH_COUNT(ph, v, sent) do { if (lane == 0 && (sent) < KB_PHASE_SENT) phaseClocks[(sent) * PH_COUNT + (ph)] += (v); } while (0)
+#else
+#define KB_PH_COUNT(ph, v, sent) do { } while (0)
+#define KB_PH_START(t) do { } while (0)
+#define KB_PH_ADD(ph, t, sent) do { } while (0)
+#endif
+
 	// a path record: DPath (kb_batch.h); the SkipBigram build appends the rest of the LM state - the ring of the last 8 valid tokens
 	// and its position - and the container hash the entry was appended with (VitView::path_stride tells emit.cu the record size)
 #if KB_SBG
@@ -537,6 +554,9 @@ namespace KB_VIT_NS
 		uint8_t uniq[2]; uint32_t nUniq;
 		uint16_t* ht; uint32_t htUsed;
 		uint32_t top1Buckets = 1;           // bucket count of the reference's `top1` unordered_set, per sentence (unordered_emu.h)
+#if KB_PHASE_CLOCKS
+		uint32_t phSent = 0;                // the sentence's index (phaseClocks)
+#endif
 #if KB_SBG
 		uint32_t sbIdxCap = 0;              // slots of the current candidate's `top1` index at the end of the sentence's pool region (0 = none yet)
 #endif
@@ -900,23 +920,26 @@ namespace KB_VIT_NS
 		// free pool slot (the segment may be followed by other candidates' entries)
 		__device__ __noinline__ uint32_t reorderTop1(uint32_t candBeg, uint32_t E, uint32_t bucketsBefore, uint32_t scratch)
 		{
+			KB_PH_START(tReorder);
 			if (E == 0) return bucketsBefore;
 			const uint32_t Bafter = unorderedBucketsAfter(bucketsBefore, E);
 			if (!Bafter) { err = ST_INTERNAL; return bucketsBefore; }
 			if (E == 1) return Bafter;
+			// (the reservation is 16 bytes per entry, of which the order takes 12; the containers that overflow the pool are the same as
+			// when the order kept 64-bit hash codes in the scratch)
 			const size_t need = (size_t)E * sizeof(PathT) + (size_t)E * 16 + (size_t)Bafter * 4;
 			if ((size_t)scratch * sizeof(PathT) + need > (size_t)poolCap * sizeof(PathT)) { err = ST_PATH_OVERFLOW; return bucketsBefore; }
 			PathT* tmp = pool + scratch;
-			unsigned long long* codes = reinterpret_cast<unsigned long long*>(pool + scratch + (size_t)E);
-			int32_t* next = reinterpret_cast<int32_t*>(codes + E); int32_t* order = next + E; int32_t* buckets = order + E;
+			int32_t* first = reinterpret_cast<int32_t*>(pool + scratch + (size_t)E); int32_t* runs = first + E; int32_t* order = runs + E; int32_t* buckets = order + E;
 			#pragma unroll 1
-			for (uint32_t e = lane; e < E; e += 32)
+			for (uint32_t e = lane; e < E; e += 32) tmp[e] = pool[candBeg + e];
+			__syncwarp();
+			// Hash<WordLL> (BestPathContainer.hpp:79-84) over Hash<LmState>: std::hash<int32_t> for Knlm (Knlm.hpp:1170-1178), Hash<uint32_t>(node) for CoNg
+			const auto codeOf = [tmp](int32_t i) -> unsigned long long
 			{
-				const PathT p = pool[candBeg + e];
-				tmp[e] = p;
-				// Hash<WordLL> (BestPathContainer.hpp:79-84) over Hash<LmState>: std::hash<int32_t> for Knlm (Knlm.hpp:1170-1178), Hash<uint32_t>(node) for CoNg
+				const PathT& p = tmp[i];
 #if KB_SBG
-				codes[e] = p.hcode;
+				return p.hcode;
 #else
 #if KB_CONG
 				const unsigned long long v = (uint32_t)p.lm_state;
@@ -924,17 +947,21 @@ namespace KB_VIT_NS
 #else
 				unsigned long long h = (unsigned long long)(long long)p.lm_state;
 #endif
-				codes[e] = (unsigned long long)((uint32_t)p.prev_root_id | ((uint32_t)p.sp_state << 8)) ^ ((h << 3) | (h >> 61));
+				return (unsigned long long)((uint32_t)p.prev_root_id | ((uint32_t)p.sp_state << 8)) ^ ((h << 3) | (h >> 61));
 #endif
-			}
-			__syncwarp();
+			};
 			uint32_t B = bucketsBefore;
-			if (lane == 0) { if (!unorderedSetOrder(codes, (int32_t)E, B, next, buckets, order)) order[0] = -1; }
-			__syncwarp();
-			if (order[0] < 0) { err = ST_INTERNAL; return bucketsBefore; }
+			KB_PH_START(tOrder);
+			if (!unorderedSetOrderWarp(codeOf, (int32_t)E, B, first, runs, buckets, order, lane)) { err = ST_INTERNAL; return bucketsBefore; }
+			KB_PH_ADD(PH_TOP1_ORDER, tOrder, phSent);
+			KB_PH_COUNT(PH_N_TOP1, 1, phSent); KB_PH_COUNT(PH_SUM_E, E, phSent); KB_PH_COUNT(PH_SUM_B, Bafter, phSent);
+#if KB_PHASE_CLOCKS
+			for (uint32_t b = bucketsBefore == 1 ? 13u : bucketsBefore; b != Bafter; b = unorderedNextBuckets(b)) KB_PH_COUNT(PH_REHASHES, 1, phSent);
+#endif
 			#pragma unroll 1
 			for (uint32_t j = lane; j < E; j += 32) pool[candBeg + j] = tmp[order[j]];
 			__syncwarp();
+			KB_PH_ADD(PH_TOP1_REORDER, tReorder, phSent);
 			return Bafter;
 		}
 
@@ -2075,7 +2102,7 @@ namespace KB_VIT_NS
 			if (ownLen) { uint16_t ol; uint8_t op; leftFeat(ownOff, ownLen, 0, 0, ol, op); fc.ownFw = fwOfLeft(ol, op); }
 			uint32_t nItems = 0;      // items waiting in sm->item
 			uint32_t nFw = 1;         // entries of sm->fwTab (index 0 unused)
-			auto flush = [&]() { const bool ok = flushItems(fc, nItems); nItems = 0; return ok; };
+			auto flush = [&]() { KB_PH_START(tFlush); const bool ok = flushItems(fc, nItems); KB_PH_ADD(PH_FLUSH, tFlush, phSent); nItems = 0; return ok; };
 			const bool snPoint = node.uform_len && norm[node.uform_off + node.uform_len - 1] == '.';
 			const uint32_t nWords = (P + 31) >> 5;
 			// class of lane's path in each of the first 6 words of 32 incoming paths, 5 bits each (+ which words have a path for this lane): the
@@ -2423,6 +2450,7 @@ namespace KB_VIT_NS
 
 			// prune (PathEvaluator.hpp:475-511): per root slot the best score of the paths whose morpheme has no combine socket;
 			// scores are compared as order-preserving unsigned keys, the threshold test itself stays a float comparison
+			KB_PH_START(tPrune);
 			if (leader())
 			{
 			const uint32_t cntAll = top - nodeBeg;
@@ -2479,6 +2507,7 @@ namespace KB_VIT_NS
 			}
 			top = nodeBeg + valid;
 			}
+			KB_PH_ADD(PH_PRUNE, tPrune, phSent);
 			if (teamSize > 1) { uint32_t t = top; teamBroadcast(t); top = t; }
 		}
 
@@ -2582,6 +2611,7 @@ namespace KB_VIT_NS
 			if (N > 2) { const uint2 c1 = nodeCand[1]; pfIssue(c_m.cands + c1.x, min(c1.y & 0xFFFFu, GROUP), curBuf ^ 1u); }
 #endif
 
+			KB_PH_START(tNodes);
 			for (uint32_t i = 1; i + 1 < N; ++i)
 			{
 				const DNode node = nodes[i];
@@ -2631,13 +2661,16 @@ namespace KB_VIT_NS
 						ol = node.end_pos - node.start_pos; oo = node.start_pos;
 						cb = c_m.cands + c_m.cand_unk; cn = 2; disc = unkFormScore(norm + node.start_pos, ol);
 					}
+					KB_PH_START(tEval);
 					evaluate(i, nodeBeg, cb, cn, disc, oo, ol, inBeg, inEnd, pass == 0);
+					KB_PH_ADD(PH_EVALUATE, tEval, phSent);
 					if (err) return 0;
 				}
 				if (lane == 0 && leader()) { npOff[i] = nodeBeg; npCnt[i] = top - nodeBeg; }
 				__syncwarp();
 				teamSync();
 			}
+			KB_PH_ADD(PH_NODE_LOOP, tNodes, phSent);
 			if (!leader()) return 0;      // the end node and the stitching are the first warp's; the others wait for its broadcast
 
 			// ---- end node (PathEvaluator.hpp:1320-1357): candidates go to the pool tail as temporary records
@@ -2863,6 +2896,9 @@ namespace KB_VIT_NS
 #if KB_TEAM > 1
 		v.teamRank = teamRank; v.teamSize = teamSize; v.teamBar = 1 + teamIdx; v.tm = &teamSm[teamIdx];
 #endif
+#if KB_PHASE_CLOCKS
+		v.phSent = s;
+#endif
 		v.splitComplex = (bv.match_options >> 22) & 1; v.splitSaisiot = (bv.match_options >> 25) & 1; v.mergeSaisiot = (bv.match_options >> 26) & 1;
 		v.htClear();
 		if (lane == 0) smAll[wib].exactInsert = 0;
@@ -2898,7 +2934,9 @@ namespace KB_VIT_NS
 
 			PathRes res[MAX_RESULTS];
 			// AnalyzeOption::openEnding (bit 31 of the option word, capi.cu): no end-of-sentence step on the chunk that ends the text (src/Kiwi.cpp:1122-1131)
+			KB_PH_START(tFind);
 			const uint32_t K = v.findBestPath(ch, res, (bv.match_options >> 31) != 0 && ch.end == normLen);
+			KB_PH_ADD(PH_FIND_BEST_PATH, tFind, s);
 
 			// ---- insertPathIntoResults, topN == 1 (src/Kiwi.cpp:629-782), all lanes redundantly (team mode: the first warp's lanes)
 			auto stitch = [&]()
@@ -3116,3 +3154,14 @@ namespace KB_VIT_NS
 #endif
 	}
 }
+
+#if KB_PHASE_CLOCKS && !KB_CONG && !KB_SBG && !defined(KB_HOSTSIM)
+// diagnostic build only: copies phaseClocks ([KB_PHASE_SENT][PH_COUNT] cycles) to `out` and zeroes them
+extern "C" __attribute__((visibility("default"))) int kiwi_b200_debug_phase_clocks(unsigned long long* out)
+{
+	using namespace kb::vit_knlm;
+	static unsigned long long zero[KB_PHASE_SENT * PH_COUNT];
+	if (cudaDeviceSynchronize() || cudaMemcpyFromSymbol(out, phaseClocks, sizeof(zero)) || cudaMemcpyToSymbol(phaseClocks, zero, sizeof(zero))) return -1;
+	return PH_COUNT;
+}
+#endif
