@@ -327,6 +327,19 @@ namespace kb
 		pack_kernel<<<blocks, threads, 0, st>>>(n, sc.bv.text_off, sc.vv.n_tokens, sc.tokOff, sc.vv.tokens, sc.packed);
 		ck(cudaGetLastError(), "pack_kernel launch");
 		ck(cudaEventRecord(ev[4], st), "event");
+		last.kernelLaunches += 6;
+	}
+
+	// CUDA-event times of the launch whose events launchAll recorded into ev[1..4]
+	struct KernelMs { float lattice = 0, viterbi = 0, pack = 0, total = 0; };
+	static KernelMs kernelMs(const cudaEvent_t* ev)
+	{
+		KernelMs t;
+		cudaEventElapsedTime(&t.lattice, ev[1], ev[2]);
+		cudaEventElapsedTime(&t.viterbi, ev[2], ev[3]);
+		cudaEventElapsedTime(&t.pack, ev[3], ev[4]);
+		cudaEventElapsedTime(&t.total, ev[1], ev[4]);
+		return t;
 	}
 
 	// KIWI_B200_SOLO=<blocks>,<warps> (work-queue kernel build): the first <blocks> blocks of the Viterbi wave keep only <warps> warps,
@@ -380,6 +393,23 @@ namespace kb
 	//    copy then and does not wait for it (drainTokenCopies at the end of the call, or before the array has to grow).
 	static size_t tokenEstimate(size_t rawUnits, uint32_t n) { return rawUnits * 5 / 8 + 8 * (size_t)n + 64; }
 
+	// End of the pass that starts at sentence i0 of the batch offsets[0..n]: sentences (W_s = 2 n_s + 4 units each) are added while
+	// fits(units, sentences) holds for the pass with them; the first one is always taken.
+	template<class Fits> static uint32_t passEnd(const uint32_t* offsets, uint32_t i0, uint32_t n, Fits fits)
+	{
+		uint32_t i1 = i0;
+		for (size_t units = 0; i1 < n; ++i1)
+		{
+			const size_t u = 2 * (size_t)(offsets[i1 + 1] - offsets[i1]) + 4;
+			if (i1 > i0 && !fits(units + u, (size_t)(i1 - i0) + 1)) break;
+			units += u;
+		}
+		return i1;
+	}
+
+	// a sentence that overflowed an arena may fit a larger one; a chunk beyond the 16-bit node index (ST_TOO_LONG) fits none
+	static bool retryable(uint32_t status) { return status && status != ST_TOO_LONG; }
+
 	void Engine::submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t pn, uint32_t matchOptions, DToken* directDst)
 	{
 		const size_t t0 = off[i0], pT = off[i0 + pn] - t0;
@@ -405,9 +435,8 @@ namespace kb
 		ck(cudaMemcpyAsync(hDbg + 1, model.dev.debug, 4, cudaMemcpyDeviceToHost, s.stream), "D2H debug");
 		if (est) ck(cudaMemcpyAsync(directDst, s.sc.packed, est * sizeof(DToken), cudaMemcpyDeviceToHost, s.stream), "D2H tokens");
 		ck(cudaEventRecord(s.ev[5], s.stream), "event");
-		s.busy = true; s.i0 = i0; s.n = pn; s.rawUnits = pT; s.units = U; s.tokCopied = est;
+		s.busy = true; s.n = pn; s.tokCopied = est;
 		last.h2dBytes += pT * 2 + ((size_t)pn + 1) * 4;
-		last.kernelLaunches += 6;
 	}
 
 	// waits for the token copies still in flight into `out.tokens` (their time counts as D2H)
@@ -424,7 +453,7 @@ namespace kb
 	}
 
 	// waits for the slot's pass, appends its sentences (they are the next ones in input order) to `out`
-	void Engine::finishPass(Slot& s, BatchOutput& out, std::vector<uint32_t>& failed)
+	void Engine::finishPass(Slot& s, BatchOutput& out)
 	{
 		if (!s.busy) return;
 		ck(cudaStreamSynchronize(s.stream), "sync (a kernel fault surfaces here)");
@@ -457,88 +486,98 @@ namespace kb
 		{
 			out.tokOff.push_back((uint32_t)(base + hTokOff[k + 1]));
 			out.scores.push_back(hScore[k]); out.status.push_back(hStatus[k]);
-			if (hStatus[k] && hStatus[k] != ST_TOO_LONG) failed.push_back(s.i0 + k);      // (a chunk beyond the 16-bit node index does not fit any arena)
 		}
+		const KernelMs t = kernelMs(s.ev);
+		out.msLattice += t.lattice; out.msViterbi += t.viterbi; out.msPack += t.pack;
 		float ms;
 		cudaEventElapsedTime(&ms, s.ev[0], s.ev[1]); out.msH2D += ms;
-		cudaEventElapsedTime(&ms, s.ev[1], s.ev[2]); out.msLattice += ms;
-		cudaEventElapsedTime(&ms, s.ev[2], s.ev[3]); out.msViterbi += ms;
-		cudaEventElapsedTime(&ms, s.ev[3], s.ev[4]); out.msPack += ms;
 		cudaEventElapsedTime(&ms, s.ev[4], s.ev[5]); out.msD2H += ms;
 		cudaEventElapsedTime(&ms, s.ev[0], s.ev[5]); out.msTotal += ms;
 		last.d2hBytes += headWords * 4 + (size_t)std::max<size_t>(total, s.tokCopied) * sizeof(DToken);
 	}
 
 	// Sentences that overflowed the arithmetic capacity of a main arena are re-run in the retry arena with 8 x the path and 4 x the
-	// node capacity, then (what still fails) with 64 x / 16 x; every round is cut into sub-passes that fit a memory budget.  What
-	// fails even then keeps its status: the caller reports it per sentence instead of failing the whole batch.
-	void Engine::runRetry(const uint16_t* text, const uint32_t* offsets, const std::vector<uint32_t>& failedIn, uint32_t matchOptions, BatchOutput& out,
-		std::vector<PassResult>& results, std::vector<uint32_t>& resultOf)
+	// node capacity (round 0), then, what still fails, with 64 x / 16 x (round 1); a round is cut into sub-passes that fit a memory
+	// budget.  runRetry runs round `round` and the rounds after it over the n sentences of the contiguous sub-batch text / offsets:
+	// `out.status` holds on entry the status each of them failed with, and `out` receives their results.  A sentence that fails even
+	// then keeps its status and has no tokens: the caller reports it per sentence instead of failing the whole batch.
+	void Engine::runRetry(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, int round, BatchOutput& out)
 	{
-		std::vector<uint32_t> failed = failedIn;
 		static const uint32_t pathMul[2] = { 8, 64 }, nodeMul[2] = { 4, 16 };
 		const size_t budget = (size_t)4 << 30;       // bytes of path pool per sub-pass (the retry arena stays allocated with its handle)
+		const uint32_t ppu = DEFAULT_PATHS_PER_UNIT * pathScale() * pathMul[round], pc = DEFAULT_PATHS_CONST * pathScale() * pathMul[round], npu = KB_DEFAULT_NODES_PER_UNIT * nodeMul[round];
+		const auto fits = [&](size_t units, size_t count) { return (units * ppu + count * pc) * pathStride() <= budget; };
 		Slot& s = slot_[0];
-		for (int round = 0; round < 2 && !failed.empty(); ++round)
+		out.tokOff.assign(1, 0); out.tokens.clear(); out.scores.assign(n, 0.f);
+		std::vector<uint32_t> subOff, tokOff;
+		for (uint32_t i0 = 0, i1; i0 < n; i0 = i1)
 		{
-			const uint32_t ppu = DEFAULT_PATHS_PER_UNIT * pathScale() * pathMul[round], pc = DEFAULT_PATHS_CONST * pathScale() * pathMul[round], npu = KB_DEFAULT_NODES_PER_UNIT * nodeMul[round];
-			std::vector<uint32_t> still;
-			size_t f0 = 0;
-			while (f0 < failed.size())
+			i1 = passEnd(offsets, i0, n, fits);
+			const uint32_t pn = i1 - i0;
+			const size_t t0 = offsets[i0], pT = offsets[i1] - t0, U = 2 * pT + 4 * (size_t)pn;
+			try { ensureScratch(retry_, s.stream, U, pn, ppu, pc, npu); }
+			catch (const std::exception&)
 			{
-				size_t f1 = f0, units = 0;
-				while (f1 < failed.size())
-				{
-					const size_t u = 2 * (size_t)(offsets[failed[f1] + 1] - offsets[failed[f1]]) + 4;
-					if (f1 > f0 && ((units + u) * ppu + (f1 - f0 + 1) * (size_t)pc) * pathStride() > budget) break;
-					units += u; ++f1;
-				}
-				std::vector<uint16_t> subText; std::vector<uint32_t> subOff{ 0 };
-				for (size_t k = f0; k < f1; ++k)
-				{
-					const uint32_t id = failed[k];
-					subText.insert(subText.end(), text + offsets[id], text + offsets[id + 1]);
-					subOff.push_back((uint32_t)subText.size());
-				}
-				const uint32_t pn = (uint32_t)(f1 - f0);
-				const size_t pT = subText.size(), U = 2 * pT + 4 * (size_t)pn;
-				try { ensureScratch(retry_, s.stream, U, pn, ppu, pc, npu); }
-				catch (const std::exception&)
-				{
-					// the escalated arena does not fit the device: these sentences keep their overflow status (no tokens), the batch goes on
-					cudaGetLastError();
-					freeScratch(retry_);
-					f0 = f1;
-					continue;
-				}
-				ck(cudaMemcpyAsync(retry_.dText, subText.data(), pT * 2, cudaMemcpyHostToDevice, s.stream), "H2D text");
-				ck(cudaMemcpyAsync(retry_.dOff, subOff.data(), ((size_t)pn + 1) * 4, cudaMemcpyHostToDevice, s.stream), "H2D offsets");
-				bind(retry_, retry_.dText, retry_.dOff, pn, matchOptions, nodeMul[round]);
-				launchAll(retry_, s.stream, s.ev, pn);
-				PassResult r;
-				r.tokOff.resize(pn + 1); r.scores.resize(pn); r.status.resize(pn);
-				ck(cudaMemcpyAsync(r.tokOff.data(), retry_.tokOff, ((size_t)pn + 1) * 4, cudaMemcpyDeviceToHost, s.stream), "D2H offsets");
-				ck(cudaMemcpyAsync(r.scores.data(), retry_.vv.score, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H scores");
-				ck(cudaMemcpyAsync(r.status.data(), retry_.bv.status, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H status");
-				ck(cudaStreamSynchronize(s.stream), "sync (retry pass)");
-				checkDebug(retry_);
-				r.toks.resize(r.tokOff[pn]);
-				if (!r.toks.empty()) ck(cudaMemcpy(r.toks.data(), retry_.packed, r.toks.size() * sizeof(DToken), cudaMemcpyDeviceToHost), "D2H tokens");
-				float ms = 0; cudaEventElapsedTime(&ms, s.ev[1], s.ev[4]); out.msTotal += ms;
-				last.h2dBytes += pT * 2 + ((size_t)pn + 1) * 4; last.d2hBytes += ((size_t)pn * 3 + 1) * 4 + r.toks.size() * sizeof(DToken); last.kernelLaunches += 6;
-				const uint32_t ri = (uint32_t)results.size();
-				for (uint32_t k = 0; k < pn; ++k)
-				{
-					const uint32_t id = failed[f0 + k];
-					out.status[id] = r.status[k];
-					if (r.status[k]) still.push_back(id);
-					else resultOf[id] = (ri << 16) | k;          // sub-passes hold < 65536 sentences (MAX_SENT_PER_PASS)
-				}
-				results.push_back(std::move(r));
-				f0 = f1;
+				// the escalated arena does not fit the device: these sentences keep their overflow status (no tokens), the batch goes on
+				cudaGetLastError();
+				freeScratch(retry_);
+				out.tokOff.resize(out.tokOff.size() + pn, (uint32_t)out.tokens.size());
+				continue;
 			}
-			failed.swap(still);
+			subOff.resize((size_t)pn + 1);
+			for (uint32_t k = 0; k <= pn; ++k) subOff[k] = offsets[i0 + k] - (uint32_t)t0;
+			ck(cudaMemcpyAsync(retry_.dText, text + t0, pT * 2, cudaMemcpyHostToDevice, s.stream), "H2D text");
+			ck(cudaMemcpyAsync(retry_.dOff, subOff.data(), ((size_t)pn + 1) * 4, cudaMemcpyHostToDevice, s.stream), "H2D offsets");
+			bind(retry_, retry_.dText, retry_.dOff, pn, matchOptions, nodeMul[round]);
+			launchAll(retry_, s.stream, s.ev, pn);
+			tokOff.resize((size_t)pn + 1);
+			ck(cudaMemcpyAsync(tokOff.data(), retry_.tokOff, ((size_t)pn + 1) * 4, cudaMemcpyDeviceToHost, s.stream), "D2H offsets");
+			ck(cudaMemcpyAsync(out.scores.data() + i0, retry_.vv.score, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H scores");
+			ck(cudaMemcpyAsync(out.status.data() + i0, retry_.bv.status, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H status");
+			ck(cudaStreamSynchronize(s.stream), "sync (retry pass)");
+			checkDebug(retry_);
+			const size_t base = out.tokens.size(), nTok = tokOff[pn];
+			out.tokens.resize(base + nTok);
+			if (nTok) ck(cudaMemcpy(out.tokens.data() + base, retry_.packed, nTok * sizeof(DToken), cudaMemcpyDeviceToHost), "D2H tokens");
+			for (uint32_t k = 1; k <= pn; ++k) out.tokOff.push_back((uint32_t)(base + tokOff[k]));
+			out.msTotal += kernelMs(s.ev).total;
+			last.h2dBytes += pT * 2 + ((size_t)pn + 1) * 4; last.d2hBytes += ((size_t)pn * 3 + 1) * 4 + nTok * sizeof(DToken);
 		}
+		if (round + 1 < 2) retryFailed(text, offsets, matchOptions, round + 1, out);
+	}
+
+	// Gathers the retryable sentences of `out` (the results of the batch text / offsets), in input order, into one contiguous
+	// sub-batch, runs it through retry round `round` and the rounds after it, and puts the results in their places.  Returns how many
+	// sentences it re-ran.
+	size_t Engine::retryFailed(const uint16_t* text, const uint32_t* offsets, uint32_t matchOptions, int round, BatchOutput& out)
+	{
+		std::vector<uint32_t> ids;
+		for (uint32_t i = 0; i < (uint32_t)out.status.size(); ++i) if (retryable(out.status[i])) ids.push_back(i);
+		if (ids.empty()) return 0;
+		std::vector<uint16_t> subText; std::vector<uint32_t> subOff{ 0 };
+		BatchOutput sub;
+		for (uint32_t id : ids)
+		{
+			subText.insert(subText.end(), text + offsets[id], text + offsets[id + 1]);
+			subOff.push_back((uint32_t)subText.size());
+			sub.status.push_back(out.status[id]);
+		}
+		runRetry(subText.data(), subOff.data(), (uint32_t)ids.size(), matchOptions, round, sub);
+		// splice the retried sentences into the token stream (rare path: rebuild)
+		TokenVec toks; std::vector<uint32_t> tokOff(1, 0);
+		toks.reserve(out.tokens.size() + sub.tokens.size());
+		for (uint32_t i = 0, k = 0; i < (uint32_t)out.status.size(); ++i)
+		{
+			const bool retried = k < ids.size() && ids[k] == i;
+			const BatchOutput& src = retried ? sub : out;
+			const uint32_t j = retried ? k++ : i;
+			toks.insert(toks.end(), src.tokens.begin() + src.tokOff[j], src.tokens.begin() + src.tokOff[j + 1]);
+			out.scores[i] = src.scores[j]; out.status[i] = src.status[j];
+			tokOff.push_back((uint32_t)toks.size());
+		}
+		out.tokens.swap(toks); out.tokOff.swap(tokOff);
+		out.msTotal += sub.msTotal;
+		return ids.size();
 	}
 
 	// Public entry: batches of any size.  The scratch arenas are sized per pass, so a large batch (65536 / 1 M sentences)
@@ -566,28 +605,22 @@ namespace kb
 		for (uint32_t i = 0; i < n; ++i) if (offsets[i + 1] < offsets[i]) throw std::runtime_error("offsets must be non-decreasing");
 		out.tokOff.reserve((size_t)n + 1); out.scores.reserve(n); out.status.reserve(n);
 		out.tokens.reserve(tokenEstimate(offsets[n], n));
-		std::vector<uint32_t> failed;
 		const size_t sentLimit = std::max<size_t>(passSentLimit() / passDivisor(), 1), unitLimit = MAX_UNITS_PER_PASS / passDivisor();
+		const auto fits = [&](size_t units, size_t count) { return units <= unitLimit && count <= sentLimit; };
 		uint32_t i0 = 0, k = 0;
 		try
 		{
 			while (i0 < n)
 			{
-				uint32_t i1 = i0; size_t units = 0;
-				while (i1 < n && i1 - i0 < sentLimit)
-				{
-					const size_t u = 2 * (size_t)(offsets[i1 + 1] - offsets[i1]) + 4;
-					if (i1 > i0 && units + u > unitLimit) break;
-					units += u; ++i1;
-				}
+				const uint32_t i1 = passEnd(offsets, i0, n, fits);
 				Slot& s = slot_[k & 1];
 				// results are appended in input order: the slot's previous pass (k - 2) is older than the other slot's (k - 1)
-				finishPass(s, out, failed);
+				finishPass(s, out);
 				submitPass(s, text, offsets, i0, i1 - i0, matchOptions, k == 0 ? out.tokens.data() : nullptr);      // (capacity reserved above)
 				i0 = i1; ++k;
 			}
-			finishPass(slot_[k & 1], out, failed);
-			finishPass(slot_[(k + 1) & 1], out, failed);
+			finishPass(slot_[k & 1], out);
+			finishPass(slot_[(k + 1) & 1], out);
 			drainTokenCopies(out);
 		}
 		catch (...)
@@ -595,28 +628,7 @@ namespace kb
 			for (auto& sl : slot_) { if (sl.busy || sl.tokPending) { cudaStreamSynchronize(sl.stream); sl.busy = false; sl.tokPending = false; } }
 			throw;
 		}
-		last.retried += failed.size();
-		if (!failed.empty())
-		{
-			std::vector<PassResult> results; std::vector<uint32_t> resultOf(n, 0xFFFFFFFFu);
-			runRetry(text, offsets, failed, matchOptions, out, results, resultOf);
-			// splice the retried sentences into the token stream (rare path: rebuild)
-			TokenVec toks; std::vector<uint32_t> tokOff(1, 0);
-			toks.reserve(out.tokens.size());
-			for (uint32_t i = 0; i < n; ++i)
-			{
-				if (resultOf[i] != 0xFFFFFFFFu)
-				{
-					const PassResult& r = results[resultOf[i] >> 16]; const uint32_t kk = resultOf[i] & 0xFFFF;
-					toks.insert(toks.end(), r.toks.begin() + r.tokOff[kk], r.toks.begin() + r.tokOff[kk + 1]);
-					out.scores[i] = r.scores[kk];
-				}
-				else if (!out.status[i]) toks.insert(toks.end(), out.tokens.begin() + out.tokOff[i], out.tokens.begin() + out.tokOff[i + 1]);
-				else out.scores[i] = 0.f;      // failed even in the escalated arena: no tokens, status kept
-				tokOff.push_back((uint32_t)toks.size());
-			}
-			out.tokens.swap(toks); out.tokOff.swap(tokOff);
-		}
+		last.retried = retryFailed(text, offsets, matchOptions, 0, out);
 		last.nSentences = n; last.rawUnits = offsets[n]; last.tokens = out.tokens.size();
 		last.msLattice = out.msLattice; last.msViterbi = out.msViterbi; last.msPack = out.msPack;
 	}
@@ -640,6 +652,7 @@ namespace kb
 		const size_t Uall = 2 * (size_t)totalUnits + 4 * (size_t)n;
 		const size_t devUnits = 4 * MAX_UNITS_PER_PASS / passDivisor(), devSent = 4 * MAX_SENT_PER_PASS / passDivisor();
 		const bool single = Uall <= devUnits && n <= devSent;      // (one launch set keeps the longest-first order over the whole batch)
+		const auto fits = [&](size_t units, size_t count) { return units <= devUnits && count <= devSent; };
 		if (!single)
 		{
 			off.resize((size_t)n + 1);
@@ -647,23 +660,12 @@ namespace kb
 		}
 		float msTotal = 0; uint64_t total = 0;
 		std::vector<uint32_t> failed;
-		uint32_t i0 = 0;
-		while (i0 < n)
+		BatchOutput retry;      // (retry.status: the status each failed sentence came back with)
+		for (uint32_t i0 = 0, i1; i0 < n; i0 = i1)
 		{
-			uint32_t i1 = n; size_t pT = totalUnits;
-			if (!single)
-			{
-				i1 = i0; size_t units = 0;
-				while (i1 < n && i1 - i0 < devSent)
-				{
-					const size_t u = 2 * (size_t)(off[i1 + 1] - off[i1]) + 4;
-					if (i1 > i0 && units + u > devUnits) break;
-					units += u; ++i1;
-				}
-				pT = off[i1] - off[i0];
-			}
+			i1 = single ? n : passEnd(off.data(), i0, n, fits);
 			const uint32_t pn = i1 - i0;
-			const size_t U = 2 * pT + 4 * (size_t)pn;
+			const size_t pT = single ? totalUnits : off[i1] - off[i0], U = 2 * pT + 4 * (size_t)pn;
 			ensureScratch(s.sc, s.stream, U, pn, DEFAULT_PATHS_PER_UNIT * pathScale(), DEFAULT_PATHS_CONST * pathScale(), KB_DEFAULT_NODES_PER_UNIT);
 			const uint16_t* pText = dText; const uint32_t* pOff = dOffsets;
 			if (!single)
@@ -679,34 +681,28 @@ namespace kb
 			ck(cudaMemcpyAsync(hTotal, s.sc.tokOff + pn, 4, cudaMemcpyDeviceToHost, s.stream), "D2H total");
 			ck(cudaMemcpyAsync(hStatus, s.sc.bv.status, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H status");
 			ck(cudaStreamSynchronize(s.stream), "sync (a kernel fault surfaces here)");
-			float a = 0;
-			cudaEventElapsedTime(&a, s.ev[1], s.ev[4]); msTotal += a;
-			cudaEventElapsedTime(&a, s.ev[1], s.ev[2]); last.msLattice += a;
-			cudaEventElapsedTime(&a, s.ev[2], s.ev[3]); last.msViterbi += a;
-			cudaEventElapsedTime(&a, s.ev[3], s.ev[4]); last.msPack += a;
+			const KernelMs t = kernelMs(s.ev);
+			msTotal += t.total; last.msLattice += t.lattice; last.msViterbi += t.viterbi; last.msPack += t.pack;
 			total += *hTotal;
-			last.kernelLaunches += 6; last.d2hBytes += 4 + (size_t)pn * 4;
-			for (uint32_t k = 0; k < pn; ++k) if (hStatus[k]) failed.push_back(i0 + k);
-			i0 = i1;
+			last.d2hBytes += 4 + (size_t)pn * 4;
+			for (uint32_t k = 0; k < pn; ++k) if (retryable(hStatus[k])) { failed.push_back(i0 + k); retry.status.push_back(hStatus[k]); }
 		}
 		last.nSentences = n; last.rawUnits = totalUnits; last.retried = failed.size();
 		if (!failed.empty())
 		{
 			// overflowed sentences (rare) go through the escalating retry arena; their text comes back from the device
 			if (off.empty()) { off.resize((size_t)n + 1); ck(cudaMemcpy(off.data(), dOffsets, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost), "D2H offsets"); }
-			std::vector<uint16_t> subText; std::vector<uint32_t> subOff{ 0 }, ids;
+			std::vector<uint16_t> subText; std::vector<uint32_t> subOff{ 0 };
 			for (uint32_t id : failed)
 			{
 				const size_t len = off[id + 1] - off[id], at = subText.size();
 				subText.resize(at + len);
 				if (len) ck(cudaMemcpy(subText.data() + at, dText + off[id], len * 2, cudaMemcpyDeviceToHost), "D2H text");
-				subOff.push_back((uint32_t)subText.size()); ids.push_back((uint32_t)ids.size());
+				subOff.push_back((uint32_t)subText.size());
 			}
-			BatchOutput tmp; tmp.status.assign(failed.size(), 1); tmp.scores.assign(failed.size(), 0.f);
-			std::vector<PassResult> results; std::vector<uint32_t> resultOf(failed.size(), 0xFFFFFFFFu);
-			runRetry(subText.data(), subOff.data(), ids, matchOptions, tmp, results, resultOf);
-			msTotal += tmp.msTotal;
-			for (auto& r : results) total += r.toks.size();
+			runRetry(subText.data(), subOff.data(), (uint32_t)failed.size(), matchOptions, 0, retry);
+			msTotal += retry.msTotal;
+			total += retry.tokens.size();
 		}
 		last.tokens = total;
 		if (nTokens) *nTokens = total;

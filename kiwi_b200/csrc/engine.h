@@ -145,7 +145,7 @@ namespace kb
 			uint16_t* hPinText = nullptr; uint32_t* hPinOff = nullptr; size_t pinTextCap = 0, pinOffCap = 0;
 			void* hPinOut = nullptr; size_t pinOutCap = 0;
 			// the pass in flight
-			bool busy = false; uint32_t i0 = 0, n = 0; size_t rawUnits = 0, units = 0, tokCopied = 0;
+			bool busy = false; uint32_t n = 0; size_t tokCopied = 0;
 			bool tokPending = false;      // a token copy into the caller's result array is still in flight on `stream`
 		};
 		const TypoDev* typo_ = nullptr; float typoThreshold_ = 2.5f;
@@ -159,7 +159,6 @@ namespace kb
 		void bind(Scratch& sc, const uint16_t* dText, const uint32_t* dOffsets, uint32_t n, uint32_t matchOptions, uint32_t capMul);
 		void uploadConstants();
 		void launchAll(Scratch& sc, cudaStream_t st, cudaEvent_t* ev, uint32_t n);
-		struct PassResult { std::vector<uint32_t> tokOff; TokenVec toks; std::vector<float> scores; std::vector<uint32_t> status; };
 		void submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t n, uint32_t matchOptions, DToken* directDst);
 		void drainTokenCopies(BatchOutput& out);
 		// SkipBigram states (Knlm node + 8-token history) rarely merge: 8 x the paths per sentence from the start (the first retry round of the
@@ -167,8 +166,9 @@ namespace kb
 		uint32_t pathScale() const { return model.dev.model_type == 3 ? 8u : 1u; }
 		size_t passDivisor() const { return model.dev.model_type == 3 ? 16 : 1; }
 		size_t pathStride() const { return model.dev.model_type == 3 ? 96 : sizeof(DPath); }      // SkipBigram paths carry their 8-token history (viterbi.cu PathS)
-		void finishPass(Slot& s, BatchOutput& out, std::vector<uint32_t>& failed);
-		void runRetry(const uint16_t* text, const uint32_t* offsets, const std::vector<uint32_t>& failed, uint32_t matchOptions, BatchOutput& out, std::vector<PassResult>& results, std::vector<uint32_t>& resultOf);
+		void finishPass(Slot& s, BatchOutput& out);
+		void runRetry(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, int round, BatchOutput& out);
+		size_t retryFailed(const uint16_t* text, const uint32_t* offsets, uint32_t matchOptions, int round, BatchOutput& out);
 		void checkDebug(Scratch& sc);
 	};
 
