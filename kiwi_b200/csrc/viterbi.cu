@@ -82,9 +82,12 @@ namespace KB_VIT_NS
 #if KB_PHASE_CLOCKS
 	// Diagnostic build only (`make variant VFLAGS="... -DKB_PHASE_CLOCKS"`, scripts/phase_clocks.py): clock64 cycles of the phases of
 	// each sentence's Viterbi, summed over the sentence, lane 0 of its warp, and what its `top1` containers held (count, entries, bucket
-	// count after each, rehashes); sentences with index >= KB_PHASE_SENT are not counted
+	// count after each, rehashes); sentences with index >= KB_PHASE_SENT are not counted.  Inside `evaluate`: path staging, candidate
+	// classification, the candidate walk (enumeration and everything it calls), the per-candidate path `evalGeneralCand` on `top1` nodes
+	// of more than HT_MAX_ENTRIES incoming paths ("big") and on all others, the exact group redo, and how many big nodes / candidates
 	enum { PH_TOP1_ORDER, PH_TOP1_REORDER, PH_FLUSH, PH_EVALUATE, PH_PRUNE, PH_NODE_LOOP, PH_FIND_BEST_PATH,
-	       PH_N_TOP1, PH_SUM_E, PH_SUM_B, PH_REHASHES, PH_COUNT };
+	       PH_N_TOP1, PH_SUM_E, PH_SUM_B, PH_REHASHES,
+	       PH_STAGE, PH_CLASSIFY, PH_WALK, PH_GEN_SMALL, PH_GEN_BIG, PH_REDO, PH_N_BIG_NODES, PH_N_BIG_CANDS, PH_COUNT };
 	constexpr uint32_t KB_PHASE_SENT = 8192;
 	__device__ unsigned long long phaseClocks[KB_PHASE_SENT * PH_COUNT];
 #define KB_PH_START(t) const long long t = clock64()
@@ -325,11 +328,22 @@ namespace KB_VIT_NS
 		out[0] = g_lmSteps; out[1] = g_lmDistinct;
 		g_lmSteps = g_lmDistinct = 0; g_lmPairs.clear();
 	}
+	// ... and where they were taken (scripts/lm_sites.py): flushItems, evalCand on a node of at most / more than HT_MAX_ENTRIES
+	// incoming paths (g_lmBigNode, set by evalCand), anywhere else
+	static uint64_t g_lmSite[4];
+	static bool g_lmBigNode;
+	extern "C" void hs32_lm_site_stats(uint64_t* out)
+	{
+		for (int i = 0; i < 4; ++i) { out[i] = g_lmSite[i]; g_lmSite[i] = 0; }
+	}
 #endif
-	__device__ __forceinline__ float knProgress(int32_t& nodeIdx, uint32_t next, uint32_t = 0)
+	__device__ __forceinline__ float knProgress(int32_t& nodeIdx, uint32_t next, uint32_t site = 0)
 	{
 #if defined(KB_HOSTSIM) && !KB_CONG && !KB_SBG
 		++g_lmSteps; g_lmDistinct += g_lmPairs.insert((uint64_t)(uint32_t)nodeIdx << 32 | next).second;
+		++g_lmSite[site == 1 || site == 2 ? 0 : site == 3 || site == 4 ? (g_lmBigNode ? 2 : 1) : 3];
+#else
+		(void)site;
 #endif
 		const KnRes r = knProgressV(nodeIdx, next);
 		nodeIdx = r.node;
@@ -977,6 +991,9 @@ namespace KB_VIT_NS
 			htClear();
 #if KB_SBG
 			sbIdxCap = 0;      // (the `top1` index of the previous candidate is dead)
+#endif
+#if defined(KB_HOSTSIM) && !KB_CONG && !KB_SBG
+			g_lmBigNode = P > HT_MAX_ENTRIES;
 #endif
 			const bool allowedSpaceBetweenChunk = c_m.cfg.space_tolerance > 0;
 
@@ -1685,20 +1702,19 @@ namespace KB_VIT_NS
 			htBase = top; htCount = 0;
 		}
 
-		// has a bucket of one of the group's containers reached 64 (distinct) states?  Segments: candidate k's entries follow candidate k - 1's,
-		// sm->candNew[k] of them, in first-insertion order
-		__device__ __noinline__ bool groupNeedsExact(uint32_t groupBase, uint32_t gcount, uint32_t mode)
+		// the group's candidates whose container has a bucket of 64 (distinct) states or more (bit k: candidate k).  Segments: candidate k's
+		// entries follow candidate k - 1's, sm->candNew[k] of them, in first-insertion order
+		__device__ __noinline__ uint32_t groupExactMask(uint32_t groupBase, uint32_t gcount, uint32_t mode)
 		{
 			const uint32_t cn = lane < gcount ? sm->candNew[lane] : 0;
 			const uint8_t cl = lane < gcount ? sm->cdyn[lane].cls : CLS_SKIP;
 			const unsigned big = __ballot_sync(FULL, cn >= KB_EXACT_FROM && (cl == CLS_ITEM || cl == CLS_GENERAL));
-			if (!big) return false;
-			if (mode == 0) return true;
+			if (!big || mode == 0) return big;
 			// medium mode: 4 buckets, count the largest one of every big candidate
 			uint32_t r = groupBase;
-			bool need = false;
+			uint32_t need = 0;
 			#pragma unroll 1
-			for (uint32_t k = 0; k < gcount && !need; ++k)
+			for (uint32_t k = 0; k < gcount; ++k)
 			{
 				const uint32_t cnt = sm->candNew[k];
 				if ((big >> k) & 1u)
@@ -1720,7 +1736,7 @@ namespace KB_VIT_NS
 						c0 += __popc(__ballot_sync(FULL, b == 0)); c1 += __popc(__ballot_sync(FULL, b == 1));
 						c2 += __popc(__ballot_sync(FULL, b == 2)); c3 += __popc(__ballot_sync(FULL, b == 3));
 					}
-					need = max(max(c0, c1), max(c2, c3)) >= KB_EXACT_FROM;
+					if (max(max(c0, c1), max(c2, c3)) >= KB_EXACT_FROM) need |= 1u << k;
 				}
 				r += cnt;
 			}
@@ -2051,6 +2067,69 @@ namespace KB_VIT_NS
 			if (lane == 0) sm->exactInsert = 0;
 			__syncwarp();
 		}
+
+		// (cold) only the candidates in `need` once more, item by item; the other candidates' containers never reached 64 states in a bucket,
+		// where the parallel insert is the reference's container, and keep their entries.  The re-runs append behind the group, then every
+		// segment is gathered in candidate order behind them and moved back to groupBase.  Returns false when that scratch does not fit the
+		// pool (err is clear then, nothing of the group has moved: the caller re-runs the whole group in place)
+		__device__ __noinline__ bool redoCandsExact(const DNode& node, const FlushCtx& fc, uint32_t groupBase, uint32_t gcount, uint32_t need)
+		{
+			const uint32_t cn = lane < gcount ? sm->candNew[lane] : 0;
+			uint32_t incl = cn;
+			for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(FULL, incl, d); if (lane >= (uint32_t)d) incl += t; }
+			uint32_t mySrc = groupBase + incl - cn, myCnt = cn;      // lane k: where candidate k's final entries are
+			const uint32_t groupEnd = groupBase + __shfl_sync(FULL, incl, 31);
+			top = groupEnd;
+			if (lane == 0) sm->exactInsert = 1;
+			__syncwarp();
+			#pragma unroll 1
+			for (uint32_t rem = need; rem; rem &= rem - 1)
+			{
+				const uint32_t k = __ffs(rem) - 1;
+				resetIndex();
+				const uint32_t before = top;
+				GenCtx g;
+				g.nodeIdx = fc.nodeIdx; g.inBeg = fc.inBeg; g.inEnd = fc.inEnd; g.mode = fc.mode; g.ownOff = fc.ownOff; g.ownLen = fc.ownLen; g.ownFw = fc.ownFw;
+				g.ignoreCondScore = fc.ignoreCondScore; g.spaceBefore = fc.spaceBefore != 0;
+#if KB_CONG
+				g.epFirst = fc.epFirst; g.dotCol = ((fc.dotMask >> k) & 1u) ? (int32_t)k : -1;
+#endif
+				evalGeneralCand(k, node, g);
+				if (err) break;
+				if (lane == k) { mySrc = before; myCnt = top - before; }
+			}
+			__syncwarp();
+			if (lane == 0) sm->exactInsert = 0;
+			__syncwarp();
+			uint32_t total = myCnt;
+			for (int d = 16; d > 0; d >>= 1) total += __shfl_xor_sync(FULL, total, d);
+			const uint32_t gather = top;
+			if (err == ST_PATH_OVERFLOW || gather + total > poolCap) { err = 0; top = groupEnd; resetIndex(); return false; }
+			if (err) return true;
+			// gather in candidate order, then back to groupBase (48-byte records as 3 x 16 bytes)
+			uint32_t dst = gather;
+			#pragma unroll 1
+			for (uint32_t k = 0; k < gcount; ++k)
+			{
+				const uint32_t src = __shfl_sync(FULL, mySrc, k), c = __shfl_sync(FULL, myCnt, k);
+				#pragma unroll 1
+				for (uint32_t e = lane; e < c; e += 32) pool[dst + e] = pool[src + e];
+				dst += c;
+			}
+			__syncwarp();
+			#pragma unroll 1
+			for (uint32_t e = lane; e < total; e += 32) pool[groupBase + e] = pool[gather + e];
+			__syncwarp();
+			if (lane < gcount)
+			{
+				sm->candNew[lane] = myCnt;
+				if (((need >> lane) & 1u) && sm->cdyn[lane].cls == CLS_ITEM) sm->cdyn[lane].cls = CLS_GENERAL;      // capacity and order are final
+			}
+			top = groupBase + total;
+			__syncwarp();
+			resetIndex();
+			return true;
+		}
 #endif
 
 		// ---- PathEvaluator::operator(), PathEvaluator.hpp:347-512 ------------------------------------
@@ -2096,7 +2175,10 @@ namespace KB_VIT_NS
 			FlushCtx fc;
 			fc.nodeIdx = nodeIdx; fc.inBeg = inBeg; fc.nodeTypoCost = node.typo_cost; fc.ownOff = ownOff; fc.ownLen = ownLen; fc.ownFw = 0;
 			fc.inEnd = inEnd; fc.mode = mode; fc.spaceBefore = spaceBefore ? 1u : 0u;
+			if (mode == 2 && P > HT_MAX_ENTRIES) { KB_PH_COUNT(PH_N_BIG_NODES, 1, phSent); KB_PH_COUNT(PH_N_BIG_CANDS, nCands, phSent); }
+			KB_PH_START(tStage);
 			if (itemOK) stagePaths(nodeIdx, inBeg, P);
+			KB_PH_ADD(PH_STAGE, tStage, phSent);
 			const bool itemOK2 = itemOK && !classOverflow;
 			const uint32_t nClasses = this->nClasses, classCommon = this->classCommon;
 			if (ownLen) { uint16_t ol; uint8_t op; leftFeat(ownOff, ownLen, 0, 0, ol, op); fc.ownFw = fwOfLeft(ol, op); }
@@ -2130,6 +2212,7 @@ namespace KB_VIT_NS
 					dcur = (rowsStaged && gb == 0) ? sm->dcandBuf[curBuf] : sm->dcandGen;
 #endif
 					// ---- classification, one lane per candidate (PathEvaluator.hpp:382-448 + evalSingleMorpheme head 531-560), from the static rows
+					KB_PH_START(tClassify);
 					uint32_t myPack = CLS_SKIP, myValid = 0, myCondFail = 0, mySets = 0;
 					{
 						uint8_t cls = CLS_SKIP, flags = 0;
@@ -2225,6 +2308,7 @@ namespace KB_VIT_NS
 						myPack = cls | ((uint32_t)flags << 8); myValid = cm.valid; myCondFail = cm.condFail; mySets = cm.sets;
 					}
 					__syncwarp();
+					KB_PH_ADD(PH_CLASSIFY, tClassify, phSent);
 #if KB_CONG
 					// tensor-core tile for the regular candidates of this group
 					uint32_t dotMask = 0;
@@ -2366,7 +2450,9 @@ namespace KB_VIT_NS
 #if KB_CONG
 						g.epFirst = cgn.epFirst; g.dotCol = ((dotMask >> k) & 1u) ? (int32_t)k : -1;
 #endif
+						KB_PH_START(tGen);
 						evalGeneralCand(k, node, g);
+						if (mode == 2 && P > HT_MAX_ENTRIES) KB_PH_ADD(PH_GEN_BIG, tGen, phSent); else KB_PH_ADD(PH_GEN_SMALL, tGen, phSent);
 						if (err) return;
 						if (lane == 0) sm->candNew[k] = top - before;
 						__syncwarp();
@@ -2376,16 +2462,24 @@ namespace KB_VIT_NS
 #if !KB_SBG && !defined(KB_NO_EXACT_REDO)
 					// The parallel insert above is the reference's container as long as no bucket reaches 64 states (0.02 % of the containers
 					// of the bench batches do).  Beyond that the reference's insertOptimized behaves differently (exactInsertRound): the
-					// group's output is dropped and its candidates are evaluated again, one after the other, item by item.
-					if (mode != 2 && teamSize == 1 && __any_sync(FULL, lane < gcount && sm->candNew[lane] >= KB_EXACT_FROM) && groupNeedsExact(myBase, gcount, mode))
+					// candidates whose container got there are evaluated again, one after the other, item by item.
+					if (mode != 2 && teamSize == 1 && __any_sync(FULL, lane < gcount && sm->candNew[lane] >= KB_EXACT_FROM))
 					{
-						redoGroupExact(node, fc, myBase, gcount);
-						if (err) return;
+						const uint32_t need = groupExactMask(myBase, gcount, mode);
+						if (need)
+						{
+							KB_PH_START(tRedo);
+							if (!redoCandsExact(node, fc, myBase, gcount, need)) redoGroupExact(node, fc, myBase, gcount);
+							KB_PH_ADD(PH_REDO, tRedo, phSent);
+							if (err) return;
+						}
 					}
 #endif
 					if (itemOK || mode == 2) { fixupGroup(myBase, gcount, mode, teamGroup); if (err) return; }
 					};
+					KB_PH_START(tWalk);
 					if (teamSize == 1 || teamGroup || leader()) walk();      // (one call site: the walk is the bulk of this function's code)
+					KB_PH_ADD(PH_WALK, tWalk, phSent);
 					if (teamSize == 1) { if (err) return; }
 					else if (teamGroup)
 					{

@@ -6,7 +6,10 @@ Knlm Viterbi object was built with -DKB_PHASE_CLOCKS (never the shipped one), se
   KIWI_B200_LIB=kiwi_b200/variants/libkiwi_b200_phase.so python scripts/phase_clocks.py [tag] [output directory, default .]
 
 -> <output directory>/phases_<tag>.json: per-sentence clock64 cycles of each phase (lane 0 of the sentence's warp) and the sentence's `top1`
-containers (count, entries, bucket counts, rehashes), for the 24 sentences with the longest Viterbi (%globaltimer)."""
+containers (count, entries, bucket counts, rehashes), for the 24 sentences with the longest Viterbi (%globaltimer).  Inside `evaluate`:
+path staging, candidate classification, the candidate walk (`enumeration` = the walk minus the calls it makes: flushItems, the
+per-candidate path, the exact redo and the `top1` order), the per-candidate path `evalCand` on `top1` nodes of more than 768 incoming
+paths ("big") and on the others, the exact group redo, and how many big nodes and candidates the sentence evaluated."""
 import ctypes as C, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -17,7 +20,8 @@ from tests.orc import IMAGE
 
 # the order of the PH_* enum in viterbi.cu
 PHASES = ["top1_order", "top1_reorder", "flush_items", "evaluate", "prune", "node_loop", "find_best_path",
-          "n_top1", "sum_E", "sum_B", "rehashes"]
+          "n_top1", "sum_E", "sum_B", "rehashes",
+          "stage_paths", "classify", "walk", "eval_cand_small", "eval_cand_big", "redo_exact", "n_big_nodes", "n_big_cands"]
 tag = sys.argv[1] if len(sys.argv) > 1 else "phase"
 out_dir = sys.argv[2] if len(sys.argv) > 2 else "."
 kw = kiwi_b200.Kiwi(IMAGE)
@@ -47,6 +51,10 @@ for i in np.argsort(-dur)[:24]:
                 "top1_order": share(P["top1_order"][i]), "top1_reorder": share(P["top1_reorder"][i]), "flush_items": share(P["flush_items"][i]),
                 "evaluate_rest": share(rest_eval), "prune": share(P["prune"][i]),
                 "end_node_and_setup": share(fb - P["node_loop"][i]), "outside_evaluate": share(P["node_loop"][i] - P["evaluate"][i]),
+                "stage_paths": share(P["stage_paths"][i]), "classify": share(P["classify"][i]),
+                "enumeration": share(P["walk"][i] - P["flush_items"][i] - P["eval_cand_small"][i] - P["eval_cand_big"][i] - P["redo_exact"][i] - P["top1_reorder"][i]),
+                "eval_cand_small": share(P["eval_cand_small"][i]), "eval_cand_big": share(P["eval_cand_big"][i]), "redo_exact": share(P["redo_exact"][i]),
+                "n_big_nodes": int(P["n_big_nodes"][i]), "n_big_cands": int(P["n_big_cands"][i]),
                 "n_top1": int(P["n_top1"][i]), "sum_E": int(P["sum_E"][i]), "sum_B": int(P["sum_B"][i]), "rehashes": int(P["rehashes"][i])})
 tot = {k: float(P[k].sum()) for k in PHASES}
 out = {"tag": tag, "span_ms": float((t[:, 1].max() - t[:, 0].min()) / 1e6),
