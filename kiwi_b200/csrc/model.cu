@@ -10,6 +10,7 @@
 #include <cuda_runtime.h>
 #include "kb_model.h"
 #include "engine.h"
+#include "lm_tables.h"
 
 namespace kb
 {
@@ -287,63 +288,15 @@ namespace kb
 		dcands[nFormCands] = makeCand(T_nng + 1u, false);          // getDefaultMorphemeId, Kiwi.h:64-67
 		dcands[nFormCands + 1] = makeCand(T_nnp + 1u, false);
 
-		// ---- Knlm one-probe layout
+		// ---- Knlm and CoNg one-probe layouts (lm_tables.h): the fourth word of an entry is the child's ll / context id for an inner
+		// edge and the state after the edge for a leaf, so no LM step walks a suffix chain on the device
 		const kb2_kn_node* knNodes = reinterpret_cast<const kb2_kn_node*>(sec(KB2_SEC_KN_NODES));
-		const uint32_t* knKeys = reinterpret_cast<const uint32_t*>(sec(KB2_SEC_KN_KEYS));
-		const int32_t* knValues = reinterpret_cast<const int32_t*>(sec(KB2_SEC_KN_VALUES));
-		const int32_t* knRoot = reinterpret_cast<const int32_t*>(sec(KB2_SEC_KN_ROOT));
-		uint32_t hashSize = 1024;
-		while (hashSize < 2 * (size_t)h->kn_num_edges + 16) hashSize <<= 1;
-		std::vector<uint4> knHash(hashSize, make_uint4(0xFFFFFFFFu, 0, 0, 0));
-		std::vector<float2> knBackoff(h->kn_num_nodes);
-		for (uint32_t i = 0; i < h->kn_num_nodes; ++i)
-		{
-			const kb2_kn_node& nd = knNodes[i];
-			float2 b; std::memcpy(&b.x, &nd.lower, 4); b.y = nd.gamma;
-			knBackoff[i] = b;
-			if (i == 0) continue;
-			for (uint32_t j = 0; j < nd.num_nexts; ++j)
-			{
-				const uint32_t key = knKeys[nd.next_offset + j];
-				const int32_t v = knValues[nd.next_offset + j];
-				float cll = 0.f;
-				if (v > 0) cll = knNodes[i + v].ll;
-				uint32_t hh = knHashFn(i, key) & (hashSize - 1);
-				while (knHash[hh].x != 0xFFFFFFFFu) hh = (hh + 1) & (hashSize - 1);
-				uint32_t cb; std::memcpy(&cb, &cll, 4);
-				knHash[hh] = make_uint4(i, key, (uint32_t)v, cb);
-			}
-		}
-		std::vector<float> knRootLl(h->kn_htx_vocab, 0.f);
-		for (uint32_t tkn = 0; tkn < h->kn_htx_vocab; ++tkn) if (knRoot[tkn] > 0 && (uint32_t)knRoot[tkn] < h->kn_num_nodes) knRootLl[tkn] = knNodes[knRoot[tkn]].ll;
-
-		// ---- CoNg context trie, one-probe layout (same idea as the Knlm table above)
-		std::vector<uint4> cgHash; std::vector<int2> cgNodes;
-		uint32_t cgHashSize = 0;
+		KnTables kn = buildKnTables(h, knNodes, reinterpret_cast<const uint32_t*>(sec(KB2_SEC_KN_KEYS)), reinterpret_cast<const int32_t*>(sec(KB2_SEC_KN_VALUES)),
+		                            reinterpret_cast<const int32_t*>(sec(KB2_SEC_KN_ROOT)), h->kn_has_htx ? reinterpret_cast<const uint32_t*>(sec(KB2_SEC_KN_HTX)) : nullptr);
+		CgTables cg;
 		if (cong)
-		{
-			const kb2_cg_node* cn = reinterpret_cast<const kb2_cg_node*>(sec(KB2_SEC_CG_NODES));
-			const uint32_t* ck = reinterpret_cast<const uint32_t*>(sec(KB2_SEC_CG_KEYS));
-			const int32_t* cv = reinterpret_cast<const int32_t*>(sec(KB2_SEC_CG_VALUES));
-			cgHashSize = 1024;
-			while (cgHashSize < 2 * (size_t)h->cg_num_edges + 16) cgHashSize <<= 1;
-			cgHash.assign(cgHashSize, make_uint4(0xFFFFFFFFu, 0, 0, 0));
-			cgNodes.resize(h->cg_num_nodes);
-			for (uint32_t i = 0; i < h->cg_num_nodes; ++i)
-			{
-				cgNodes[i] = make_int2(cn[i].lower, (int32_t)cn[i].value);
-				if (i == 0) continue;
-				for (uint32_t j = 0; j < cn[i].num_nexts; ++j)
-				{
-					const uint32_t key = ck[cn[i].next_offset + j];
-					const int32_t v = cv[cn[i].next_offset + j];
-					const uint32_t childCtx = v > 0 ? cn[i + v].value : 0;
-					uint32_t hh = knHashFn(i, key) & (cgHashSize - 1);
-					while (cgHash[hh].x != 0xFFFFFFFFu) hh = (hh + 1) & (cgHashSize - 1);
-					cgHash[hh] = make_uint4(i, key, (uint32_t)v, childCtx);
-				}
-			}
-		}
+			cg = buildCgTables(h, reinterpret_cast<const kb2_cg_node*>(sec(KB2_SEC_CG_NODES)), reinterpret_cast<const uint32_t*>(sec(KB2_SEC_CG_KEYS)),
+			                   reinterpret_cast<const int32_t*>(sec(KB2_SEC_CG_VALUES)), reinterpret_cast<const int32_t*>(sec(KB2_SEC_CG_ROOT)));
 
 		// ---- upload
 		void* dBlob = nullptr;
@@ -371,17 +324,17 @@ namespace kb
 		d.cands = upload(dcands, owned); d.cand_unk = nFormCands;
 		hCands = dcands;
 		d.chunk_lm = upload(chunkLm, owned);
-		d.kn_hash = upload(knHash, owned); d.kn_hash_mask = hashSize - 1;
-		d.kn_backoff = upload(knBackoff, owned);
-		d.kn_root_ll = upload(knRootLl, owned);
+		d.kn_hash = upload(kn.hash, owned); d.kn_hash_mask = (uint32_t)kn.hash.size() - 1;
+		d.kn_backoff = upload(kn.backoff, owned);
+		d.kn_root_ll = upload(kn.rootLl, owned);
 		d.forms = upload(dforms, owned);
 		d.chr_bmp = upload(bmp, owned);
 		d.trie_root_next = upload(rootNext, owned);
 		d.model_type = h->model_type;
 		if (cong)
 		{
-			d.cg_hash = upload(cgHash, owned); d.cg_hash_mask = cgHashSize - 1;
-			d.cg_nodes = upload(cgNodes, owned);
+			d.cg_hash = upload(cg.hash, owned); d.cg_hash_mask = (uint32_t)cg.hash.size() - 1;
+			d.cg_nodes = upload(cg.nodes, owned);
 			d.cg_root = reinterpret_cast<const int32_t*>(dsec(KB2_SEC_CG_ROOT));
 			d.cg_ctx_emb = reinterpret_cast<const uint8_t*>(dsec(KB2_SEC_CG_CTX_EMB));
 			d.cg_out_emb = reinterpret_cast<const uint8_t*>(dsec(KB2_SEC_CG_OUT_EMB));

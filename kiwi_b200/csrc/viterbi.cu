@@ -23,6 +23,9 @@
 // Compile with -fmad=false: the reference's float sums are not contracted (x86-64 baseline, no FMA).
 #include <cstdlib>
 #ifdef KB_HOSTSIM
+#include <array>
+#include <cstdio>
+#include <unordered_map>
 #include <unordered_set>
 #endif
 #include <cuda_runtime.h>
@@ -205,120 +208,187 @@ namespace KB_VIT_NS
 	// ---- KnLangModel::progress, src/Knlm.cpp:44-130 (one lane) -------------------------------------
 	// Same arithmetic (float adds in the reference's order), different table layout: the per-node sorted key
 	// arrays + binary search of the reference become ONE probe into an open-addressing table over all edges whose
-	// entry also carries the child's ll, and the root uses direct tables (model.cu "Knlm one-probe layout").
-	__device__ __forceinline__ bool knLookup(uint32_t node, uint32_t key, int32_t& v, float& childLl)
+	// entry also carries a second word, and the root uses direct tables (lm_tables.h, built by model.cu at load).
+	// That word is returned as raw bits: the child's ll for an inner edge (v > 0), the state after the edge for a leaf (v <= 0).
+	__device__ __forceinline__ bool knLookup(uint32_t node, uint32_t key, int32_t& v, uint32_t& w)
 	{
 		uint32_t h = knHashFn(node, key) & c_m.kn_hash_mask;
 		while (true)
 		{
 			const uint4 e = c_m.kn_hash[h];
-			if (e.x == node && e.y == key) { v = (int32_t)e.z; childLl = __uint_as_float(e.w); return true; }
+			if (e.x == node && e.y == key) { v = (int32_t)e.z; w = e.w; return true; }
 			if (e.x == 0xFFFFFFFFu) return false;
 			h = (h + 1) & c_m.kn_hash_mask;
 		}
 	}
 	// (state in, {log-probability, state} out - both in registers: a reference parameter would pin the caller's state to local memory)
 	struct KnRes { float ll; int32_t node; };
-	__device__ __noinline__ KnRes knProgressV(int32_t nodeIdx, uint32_t next)
-	{
-		float acc = 0;
-		while (true)
-		{
-			int32_t v; float cll;
-			if (nodeIdx == 0)
-			{
-				v = c_m.kn_root[next];
-				if (v == 0)
-				{
-					if (c_m.kn_htx) nodeIdx = c_m.kn_root[c_m.kn_htx[next]];
-					return KnRes{ acc + c_m.kn_unk_ll, nodeIdx };
-				}
-				cll = c_m.kn_root_ll[next];
-			}
-			else
-			{
-				const float2 bo = c_m.kn_backoff[nodeIdx];            // issued together with the probe
-				if (!knLookup((uint32_t)nodeIdx, next, v, cll))
-				{
-					acc += bo.y;
-					nodeIdx += __float_as_int(bo.x);
-					continue;
-				}
-			}
-			if (v > 0)
-			{
-				nodeIdx += v;
-				return KnRes{ acc + cll, nodeIdx };
-			}
-			// leaf: next state = deepest suffix state that continues with `next`
-			int32_t cur = nodeIdx;
-			while (true)
-			{
-				const int32_t lower = __float_as_int(c_m.kn_backoff[cur].x);
-				if (!lower) break;
-				cur += lower;
-				int32_t lv; float dummy;
-				const bool found = cur == 0 ? ((lv = c_m.kn_root[next]) != 0) : knLookup((uint32_t)cur, next, lv, dummy);
-				if (found && lv > 0)
-				{
-					nodeIdx = cur + lv;
-					return KnRes{ acc + asFloat(v), nodeIdx };
-				}
-			}
-			nodeIdx = c_m.kn_htx ? c_m.kn_root[c_m.kn_htx[next]] : 0;
-			return KnRes{ acc + asFloat(v), nodeIdx };
-		}
-	}
 	__device__ __forceinline__ KnRes knProgressI(int32_t nodeIdx, uint32_t next)
 	{
 		float acc = 0;
 		while (true)
 		{
-			int32_t v; float cll;
 			if (nodeIdx == 0)
 			{
-				v = c_m.kn_root[next];
-				if (v == 0)
-				{
-					if (c_m.kn_htx) nodeIdx = c_m.kn_root[c_m.kn_htx[next]];
-					return KnRes{ acc + c_m.kn_unk_ll, nodeIdx };
-				}
-				cll = c_m.kn_root_ll[next];
+				const int32_t v = c_m.kn_root[next];
+				if (v > 0) return KnRes{ acc + c_m.kn_root_ll[next], v };
+				// unknown token (v == 0) or a leaf of the root (v < 0, whose ll it holds): the root has no suffix to fall back to
+				const int32_t st = c_m.kn_htx ? c_m.kn_root[c_m.kn_htx[next]] : 0;
+				return KnRes{ acc + (v == 0 ? c_m.kn_unk_ll : asFloat(v)), st };
 			}
-			else
+			const float2 bo = c_m.kn_backoff[nodeIdx];            // issued together with the probe
+			int32_t v; uint32_t w;
+			if (!knLookup((uint32_t)nodeIdx, next, v, w))
 			{
-				const float2 bo = c_m.kn_backoff[nodeIdx];            // issued together with the probe
-				if (!knLookup((uint32_t)nodeIdx, next, v, cll))
-				{
-					acc += bo.y;
-					nodeIdx += __float_as_int(bo.x);
-					continue;
-				}
+				acc += bo.y;
+				nodeIdx += __float_as_int(bo.x);
+				continue;
 			}
-			if (v > 0)
-			{
-				nodeIdx += v;
-				return KnRes{ acc + cll, nodeIdx };
-			}
-			// leaf: next state = deepest suffix state that continues with `next`
-			int32_t cur = nodeIdx;
-			while (true)
-			{
-				const int32_t lower = __float_as_int(c_m.kn_backoff[cur].x);
-				if (!lower) break;
-				cur += lower;
-				int32_t lv; float dummy;
-				const bool found = cur == 0 ? ((lv = c_m.kn_root[next]) != 0) : knLookup((uint32_t)cur, next, lv, dummy);
-				if (found && lv > 0)
-				{
-					nodeIdx = cur + lv;
-					return KnRes{ acc + asFloat(v), nodeIdx };
-				}
-			}
-			nodeIdx = c_m.kn_htx ? c_m.kn_root[c_m.kn_htx[next]] : 0;
-			return KnRes{ acc + asFloat(v), nodeIdx };
+			if (v > 0) return KnRes{ acc + __uint_as_float(w), nodeIdx + v };
+			return KnRes{ acc + asFloat(v), (int32_t)w };         // leaf: v holds its ll, w the next state
 		}
 	}
+	__device__ __noinline__ KnRes knProgressV(int32_t nodeIdx, uint32_t next) { return knProgressI(nodeIdx, next); }
+#if defined(KB_HOSTSIM) && !KB_SBG
+	// tests/hostsim (scripts/lm_chain.py): the serial dependent loads of every LM step, i.e. the probe slots of its chain (root table
+	// reads included; CoNg also reads a node's suffix link only after the probe missed) and its backoff levels, and the loads the
+	// kernels spent after a leaf before lm_tables.h stored the leaf's next state.  Those come in two kinds, counted apart: the suffix
+	// walk after a leaf edge of a non-root node (re-done here and checked against the stored state), and the single read of the root's
+	// empty suffix link after a leaf of the root.  Per flushItems round, the largest sum over the round's active lanes is kept three
+	// ways: with both (the kernels before), with neither (now), and with the non-root walk only.  A round lasts as long as its slowest lane.
+	struct HsChain { uint64_t steps, probes, backoffs, leafSteps, walkLevels, walkLoads, rootLeafSteps, rounds, roundMax[3]; };
+	static HsChain g_chain;
+	static uint32_t g_chainLane[512][3];           // per thread: loads of its LM steps since its round began {before, now, non-root walk only}
+	static uint32_t g_chainFlush[512];             // per thread: flushItems calls
+	static std::unordered_map<uint64_t, std::array<uint32_t, 3>> g_chainRounds;      // (warp, call, round) -> maxima over its lanes
+	static bool hsProbe(const uint4* tab, uint32_t mask, uint32_t node, uint32_t key, int32_t& v, uint32_t& w, uint32_t& loads)
+	{
+		for (uint32_t h = knHashFn(node, key) & mask;; h = (h + 1) & mask)
+		{
+			++loads;
+			const uint4 e = tab[h];
+			if (e.x == node && e.y == key) { v = (int32_t)e.z; w = e.w; return true; }
+			if (e.x == 0xFFFFFFFFu) return false;
+		}
+	}
+	// after: the step's loads now; walk: the non-root leaf walk's loads; rootLeaf: 1 when the step ended on a leaf of the root
+	static void hsChainAdd(uint32_t after, uint32_t walk, uint32_t rootLeaf)
+	{
+		++g_chain.steps; g_chain.probes += after; g_chain.walkLoads += walk; g_chain.rootLeafSteps += rootLeaf;
+		uint32_t* l = g_chainLane[threadIdx.x];
+		l[0] += after + walk + rootLeaf; l[1] += after; l[2] += after + walk;
+	}
+	static void hsChainMismatch(int32_t node, uint32_t next, uint32_t stored, int32_t walked)
+	{
+		std::fprintf(stderr, "[hs32] leaf edge (%d, %u): stored state %u, suffix walk %d\n", node, next, stored, walked);
+		std::abort();
+	}
+#if !KB_CONG
+	static void hsChainStep(int32_t node, uint32_t next)
+	{
+		uint32_t after = 0, walk = 0, rootLeaf = 0;
+		while (true)
+		{
+			if (node == 0)
+			{
+				const int32_t v = c_m.kn_root[next]; ++after;
+				if (v <= 0 && c_m.kn_htx) after += 2;                    // kn_htx[next], then its root entry
+				rootLeaf = v < 0;                                          // the kernels read the root's (empty) suffix link first
+				break;
+			}
+			int32_t v; uint32_t w;
+			if (!hsProbe(c_m.kn_hash, c_m.kn_hash_mask, (uint32_t)node, next, v, w, after))
+			{
+				++g_chain.backoffs; node += __float_as_int(c_m.kn_backoff[node].x); continue;      // link read with the probe
+			}
+			if (v > 0) break;
+			++g_chain.leafSteps;
+			int32_t cur = node, st = -1;
+			while (true)
+			{
+				++walk;                                                    // kn_backoff[cur]
+				const int32_t lower = __float_as_int(c_m.kn_backoff[cur].x);
+				if (!lower) break;
+				cur += lower; ++g_chain.walkLevels;
+				int32_t lv = 0; uint32_t lw; bool f;
+				if (cur == 0) { ++walk; f = (lv = c_m.kn_root[next]) != 0; }
+				else f = hsProbe(c_m.kn_hash, c_m.kn_hash_mask, (uint32_t)cur, next, lv, lw, walk);
+				if (f && lv > 0) { st = cur + lv; break; }
+			}
+			if (st < 0) { if (c_m.kn_htx) walk += 2; st = c_m.kn_htx ? c_m.kn_root[c_m.kn_htx[next]] : 0; }
+			if ((uint32_t)st != w) hsChainMismatch(node, next, w, st);
+			break;
+		}
+		hsChainAdd(after, walk, rootLeaf);
+	}
+	extern "C" void hs32_lm_chain_stats(uint64_t* out)
+#else
+	static void hsChainStep(int32_t node, uint32_t next)
+	{
+		uint32_t after = 0, walk = 0, rootLeaf = 0;
+		while (true)
+		{
+			if (node == 0)
+			{
+				const int32_t v = next < c_m.cg_root_size ? c_m.cg_root[next] : 0; ++after;
+				if (v > 0) ++after;                                        // cg_nodes[v].y
+				rootLeaf = v < 0;                                          // the kernels read the root's (empty) suffix link first
+				break;
+			}
+			int32_t v; uint32_t w;
+			if (!hsProbe(c_m.cg_hash, c_m.cg_hash_mask, (uint32_t)node, next, v, w, after))
+			{
+				++after; ++g_chain.backoffs;                               // cg_nodes[node].x, read after the miss
+				const int32_t lower = c_m.cg_nodes[node].x;
+				if (!lower) break;
+				node += lower; continue;
+			}
+			if (v > 0) break;
+			++g_chain.leafSteps;
+			int32_t cur = node, st = 0;
+			while (true)
+			{
+				++walk;                                                    // cg_nodes[cur].x
+				const int32_t lower = c_m.cg_nodes[cur].x;
+				if (!lower) break;
+				cur += lower; ++g_chain.walkLevels;
+				int32_t lv = 0; uint32_t lw; bool f;
+				if (cur == 0) { ++walk; lv = next < c_m.cg_root_size ? c_m.cg_root[next] : 0; f = lv != 0; }
+				else f = hsProbe(c_m.cg_hash, c_m.cg_hash_mask, (uint32_t)cur, next, lv, lw, walk);
+				if (f && lv > 0) { st = cur + lv; break; }
+			}
+			if ((uint32_t)st != w) hsChainMismatch(node, next, w, st);
+			break;
+		}
+		hsChainAdd(after, walk, rootLeaf);
+	}
+	extern "C" void hs32_cg_chain_stats(uint64_t* out)
+#endif
+	{
+		// {steps, chain loads, backoff levels, non-root leaf steps, their walk levels, their walk loads, root-leaf steps, flushItems rounds,
+		//  sums of the round maxima: before, now, non-root walk only}
+		for (const auto& r : g_chainRounds) { ++g_chain.rounds; for (int k = 0; k < 3; ++k) g_chain.roundMax[k] += r.second[k]; }
+		const uint64_t v[11] = { g_chain.steps, g_chain.probes, g_chain.backoffs, g_chain.leafSteps, g_chain.walkLevels, g_chain.walkLoads,
+		                         g_chain.rootLeafSteps, g_chain.rounds, g_chain.roundMax[0], g_chain.roundMax[1], g_chain.roundMax[2] };
+		for (int i = 0; i < 11; ++i) out[i] = v[i];
+		g_chain = HsChain{}; g_chainRounds.clear();
+	}
+	static void hsChainRound(uint32_t ib)
+	{
+		const uint32_t t = threadIdx.x;
+		auto& m = g_chainRounds[(uint64_t)(t >> 5) << 56 | (uint64_t)g_chainFlush[t] << 24 | ib];
+		for (int k = 0; k < 3; ++k) m[k] = std::max(m[k], g_chainLane[t][k]);
+	}
+#define KB_HS_CHAIN_STEP(node, next) hsChainStep((node), (next))
+#define KB_HS_CHAIN_FLUSH() (++g_chainFlush[threadIdx.x])
+#define KB_HS_CHAIN_ROUND_BEGIN() (g_chainLane[threadIdx.x][0] = g_chainLane[threadIdx.x][1] = g_chainLane[threadIdx.x][2] = 0)
+#define KB_HS_CHAIN_ROUND_END(ib) hsChainRound(ib)
+#else
+#define KB_HS_CHAIN_STEP(node, next) ((void)0)
+#define KB_HS_CHAIN_FLUSH() ((void)0)
+#define KB_HS_CHAIN_ROUND_BEGIN() ((void)0)
+#define KB_HS_CHAIN_ROUND_END(ib) ((void)0)
+#endif
 #if defined(KB_HOSTSIM) && !KB_CONG && !KB_SBG
 	// tests/hostsim: LM steps and distinct (state, wid) pairs of one sentence (scripts/lm_repeat.py reads and resets them per sentence)
 	static uint64_t g_lmSteps, g_lmDistinct;
@@ -342,6 +412,7 @@ namespace KB_VIT_NS
 #if defined(KB_HOSTSIM) && !KB_CONG && !KB_SBG
 		++g_lmSteps; g_lmDistinct += g_lmPairs.insert((uint64_t)(uint32_t)nodeIdx << 32 | next).second;
 		++g_lmSite[site == 1 || site == 2 ? 0 : site == 3 || site == 4 ? (g_lmBigNode ? 2 : 1) : 3];
+		KB_HS_CHAIN_STEP(nodeIdx, next);
 #else
 		(void)site;
 #endif
@@ -356,13 +427,14 @@ namespace KB_VIT_NS
 	static constexpr uint32_t CG_UCAP = KB_CG_UCAP;  // unique contexts of a node held in the tensor-core tile (else per-pair dp4a); 32 keeps 4 blocks per SM
 	static constexpr uint32_t CG_CANDS = KB_CG_CANDS; // candidates of one lattice node (the largest candidate list of the test models has 90 entries)
 
-	__device__ __forceinline__ bool cgLookup(uint32_t node, uint32_t key, int32_t& v, uint32_t& childCtx)
+	// as knLookup: the fourth word is the child's context id for an inner edge, the node after the edge for a leaf (lm_tables.h)
+	__device__ __forceinline__ bool cgLookup(uint32_t node, uint32_t key, int32_t& v, uint32_t& w)
 	{
 		uint32_t h = knHashFn(node, key) & c_m.cg_hash_mask;
 		while (true)
 		{
 			const uint4 e = c_m.cg_hash[h];
-			if (e.x == node && e.y == key) { v = (int32_t)e.z; childCtx = e.w; return true; }
+			if (e.x == node && e.y == key) { v = (int32_t)e.z; w = e.w; return true; }
 			if (e.x == 0xFFFFFFFFu) return false;
 			h = (h + 1) & c_m.cg_hash_mask;
 		}
@@ -375,40 +447,26 @@ namespace KB_VIT_NS
 			if (atomicCAS(&c_m.debug[0], 0u, 1u) == 0u) { c_m.debug[1] = 77; c_m.debug[2] = next; c_m.debug[3] = (uint32_t)nodeIdx; c_m.debug[4] = blockIdx.x; c_m.debug[5] = threadIdx.x; }
 			nodeIdx = 0; return 0;
 		}
+		KB_HS_CHAIN_STEP(nodeIdx, next);
 		while (true)
 		{
-			int32_t v; uint32_t cctx = 0;
-			if (nodeIdx != 0)
+			if (nodeIdx == 0)
 			{
-				if (!cgLookup((uint32_t)nodeIdx, next, v, cctx))
-				{
-					const int32_t lower = c_m.cg_nodes[nodeIdx].x;
-					if (!lower) return 0;
-					nodeIdx += lower;
-					continue;
-				}
-			}
-			else
-			{
-				v = next < c_m.cg_root_size ? c_m.cg_root[next] : 0;
+				const int32_t v = next < c_m.cg_root_size ? c_m.cg_root[next] : 0;
 				if (v == 0) return 0;
-				if (v > 0) cctx = (uint32_t)c_m.cg_nodes[v].y;
+				if (v > 0) { nodeIdx = v; return (uint32_t)c_m.cg_nodes[v].y; }
+				return (uint32_t)-v;                               // a leaf of the root: the root has no suffix, the state stays 0
 			}
-			if (v > 0) { nodeIdx += v; return cctx; }
-			// leaf: next node = deepest suffix node that continues with `next`
-			int32_t cur = nodeIdx;
-			while (true)
+			int32_t v; uint32_t w;
+			if (!cgLookup((uint32_t)nodeIdx, next, v, w))
 			{
-				const int32_t lower = c_m.cg_nodes[cur].x;
-				if (!lower) break;
-				cur += lower;
-				int32_t lv; uint32_t dummy;
-				bool found;
-				if (cur != 0) found = cgLookup((uint32_t)cur, next, lv, dummy);
-				else { lv = next < c_m.cg_root_size ? c_m.cg_root[next] : 0; found = lv != 0; }
-				if (found && lv > 0) { nodeIdx = cur + lv; return (uint32_t)-v; }
+				const int32_t lower = c_m.cg_nodes[nodeIdx].x;
+				if (!lower) return 0;
+				nodeIdx += lower;
+				continue;
 			}
-			nodeIdx = 0;
+			if (v > 0) { nodeIdx += v; return w; }
+			nodeIdx = (int32_t)w;                                 // leaf: -v is its context id, w the next node
 			return (uint32_t)-v;
 		}
 	}
@@ -1506,11 +1564,13 @@ namespace KB_VIT_NS
 			const uint32_t lane = this->lane, poolCap = this->poolCap, htBase = this->htBase;
 			const uint8_t uniq0 = uniq[0], uniq1 = uniq[1];
 			uint32_t htCount = this->htCount, htUsed = this->htUsed;
+			KB_HS_CHAIN_FLUSH();
 			__syncwarp();
 			#pragma unroll 1
 			for (uint32_t ib = 0; ib < nItems; ib += 32)
 			{
 				const uint32_t i = ib + lane;
+				KB_HS_CHAIN_ROUND_BEGIN();
 				const bool valid = i < nItems;
 				uint32_t slot = 0, q = 0, r = 0, fwIdx = 0; bool condFail = false, spacePen = false;
 				if (valid) { const uint32_t it = sm->item[i]; slot = it >> 27; fwIdx = (it >> 20) & 63; q = (it >> 3) & 0x1FFFF; spacePen = (it >> 2) & 1; r = (it >> 1) & 1; condFail = it & 1; }
@@ -1586,6 +1646,7 @@ namespace KB_VIT_NS
 						}
 					}
 #endif
+					KB_HS_CHAIN_ROUND_END(ib);
 					// RuleBasedScorer::operator() + special-state update (PathEvaluator.hpp:115-183, 208-230)
 					const uint32_t ptag = pf & MF_TAG_MASK;
 					const uint32_t specialType = (csFeat >> MF_SPECIAL_SHIFT) & 7, sbType = (csFeat >> MF_SBTYPE_SHIFT) & 31;
