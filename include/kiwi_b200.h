@@ -7,8 +7,9 @@
  * image handling, device control); everything else keeps the reference's name, argument meaning and
  * error convention (never throws across the ABI; NULL / KIWIERR_* + kiwi_error() per calling thread).
  *
- * Out of scope (SURVEY.md section 8b): builder, user-defined typo rule sets, morphset, pretokenized spans,
- * joiner, sub-word tokenizer, sentence splitter — passing a non-NULL handle for one of those is an error.
+ * Out of scope (SURVEY.md section 8b): builder, user-defined typo rule sets, pretokenized spans, joiner,
+ * sub-word tokenizer — passing a non-NULL handle for one of those is an error.  The sentence splitter
+ * (kiwi_split_into_sents[_w], kiwi_ss_*) runs its rules on the device, after the analysis.
  */
 #ifndef KIWI_B200_H
 #define KIWI_B200_H
@@ -40,6 +41,7 @@ typedef struct kiwi_morphset* kiwi_morphset_h;        /* capi.h:36 */
 typedef struct kiwi_pretokenized* kiwi_pretokenized_h;/* capi.h:37 */
 typedef struct kiwi_prepared_typo* kiwi_prepared_typo_h; /* capi.h:38 */
 typedef struct kiwi_typo* kiwi_typo_h;                   /* capi.h:35 */
+typedef struct kiwi_ss* kiwi_ss_h;                       /* capi.h:33 */
 typedef unsigned short kchar16_t;                     /* capi.h:39 */
 
 typedef struct {                                      /* capi.h:43-61 */
@@ -147,6 +149,19 @@ float kiwi_res_score(kiwi_res_h result, int index, int num);                 /* 
 float kiwi_res_typo_cost(kiwi_res_h result, int index, int num);             /* capi.h:927 */
 int kiwi_res_close(kiwi_res_h result);                                       /* capi.h:937 */
 
+/* ---- sentence splitting: Kiwi::splitIntoSents (src/Kiwi.cpp:417-450, src/capi/kiwi_c.cpp:973-1009, 1660-1720) ------------------
+ * The text is analysed top-1 with match_options (checked like kiwi_analyze_option_t::match_options) and its sentences are found on the
+ * device from the token rows (sentence rules: fillSentLineInfo, src/Kiwi.cpp:322-415).  Ranges are [begin, end) in UTF-16 units of the
+ * text (kiwi_split_into_sents_w) or in bytes of the UTF-8 text (kiwi_split_into_sents).  tokenized_res (may be NULL) receives the
+ * analysis the ranges come from, equal to what kiwi_analyze_w(text, 1, {match_options}) returns.  NULL handle: NULL; otherwise
+ * NULL + kiwi_error() on failure.  A text that overflows even the retry capacity has no tokens and no sentence. */
+kiwi_ss_h kiwi_split_into_sents_w(kiwi_h handle, const kchar16_t* text, int match_options, kiwi_res_h* tokenized_res);   /* capi.h:738 */
+kiwi_ss_h kiwi_split_into_sents(kiwi_h handle, const char* text, int match_options, kiwi_res_h* tokenized_res);          /* capi.h:752 */
+int kiwi_ss_size(kiwi_ss_h result);                                          /* capi.h:1166; KIWIERR_INVALID_HANDLE on NULL */
+int kiwi_ss_begin_position(kiwi_ss_h result, int index);                     /* capi.h:1175; KIWIERR_INVALID_INDEX out of range */
+int kiwi_ss_end_position(kiwi_ss_h result, int index);                       /* capi.h:1184 */
+int kiwi_ss_close(kiwi_ss_h result);                                         /* capi.h:1194 */
+
 /* ---- additive batched interface (flat arrays; what kiwi_analyze_mw drains into) -------------------- */
 typedef struct {
 	uint32_t morph_id;      /* morphToId(PathNode.morph) after unifyMorpheme (PathEvaluator.hpp:1054-1058) */
@@ -173,6 +188,21 @@ typedef struct {
  * (including any sentence that overflowed even the retry capacity).  Free with kiwi_b200_batch_free. */
 const kiwi_b200_batch_t* kiwi_b200_analyze_batch(kiwi_h handle, const kchar16_t* text, const uint32_t* offsets, int n, kiwi_analyze_option_t option);
 void kiwi_b200_batch_free(const kiwi_b200_batch_t* batch);
+
+/* Additive: the sentence ranges of n documents (one UTF-16 blob + offsets[n+1], as kiwi_b200_analyze_batch takes them).  Only the
+ * ranges come back from the device, not the token rows.  Document i's ranges are [sent_offsets[i], sent_offsets[i+1]) of begin / end,
+ * UTF-16 units relative to the document; a document with a non-zero status has none.  ms_sents: the sentence kernels.  NULL +
+ * kiwi_error() on failure.  Free with kiwi_b200_sents_free. */
+typedef struct {
+	int n_docs;
+	const uint32_t* sent_offsets;       /* [n_docs + 1] into begin / end */
+	const uint32_t* begin;              /* UTF-16 units, relative to the document */
+	const uint32_t* end;
+	const uint32_t* status;             /* 0 = ok */
+	float ms_h2d, ms_lattice, ms_viterbi, ms_sents, ms_d2h, ms_total;
+} kiwi_b200_sents_t;
+const kiwi_b200_sents_t* kiwi_b200_split_batch(kiwi_h handle, const kchar16_t* text, const uint32_t* offsets, int n, int match_options);
+void kiwi_b200_sents_free(const kiwi_b200_sents_t* sents);
 
 /* Same work with inputs already resident in device memory (used by bench.py's device-resident leg). The
  * text / offsets pointers are DEVICE pointers; results stay on the device; returns elapsed device ms or < 0. */

@@ -5,6 +5,7 @@ fallback, and importing/using this module on a box without the built extension o
 Mirrors (reference file:line under /root/reference/):
   Kiwi.analyze(text, top_n=1)            include/kiwi/Kiwi.h:333-400, src/Kiwi.cpp:1014-1158
   Kiwi.analyze(iterable) -> ordered list include/kiwi/Kiwi.h:402-454 (reader/receiver batch mode)
+  Kiwi.split_into_sents(text)            src/Kiwi.cpp:417-450 (Kiwi::splitIntoSents)
   Token fields                           include/kiwi/Types.h:344-391 (TokenInfo)
 """
 from __future__ import annotations
@@ -123,6 +124,12 @@ class _Batch(C.Structure):
                 ("ms_pack", C.c_float), ("ms_d2h", C.c_float), ("ms_total", C.c_float)]
 
 
+class _Sents(C.Structure):
+    _fields_ = [("n_docs", C.c_int), ("sent_offsets", C.POINTER(C.c_uint32)), ("begin", C.POINTER(C.c_uint32)), ("end", C.POINTER(C.c_uint32)),
+                ("status", C.POINTER(C.c_uint32)), ("ms_h2d", C.c_float), ("ms_lattice", C.c_float), ("ms_viterbi", C.c_float),
+                ("ms_sents", C.c_float), ("ms_d2h", C.c_float), ("ms_total", C.c_float)]
+
+
 class Stats(C.Structure):
     _fields_ = [("n_sentences", C.c_uint64), ("raw_units", C.c_uint64), ("norm_units", C.c_uint64), ("lattice_nodes", C.c_uint64),
                 ("tokens", C.c_uint64), ("paths", C.c_uint64), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("kernel_launches", C.c_uint64), ("retried", C.c_uint64),
@@ -196,6 +203,16 @@ def load_library() -> C.CDLL:
     lib.kiwi_res_tag.argtypes = [C.c_void_p, C.c_int, C.c_int]
     lib.kiwi_res_form.restype = C.c_char_p
     lib.kiwi_res_form.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    for fn, text_t in (("kiwi_split_into_sents_w", C.c_void_p), ("kiwi_split_into_sents", C.c_char_p)):
+        getattr(lib, fn).restype = C.c_void_p
+        getattr(lib, fn).argtypes = [C.c_void_p, text_t, C.c_int, C.POINTER(C.c_void_p)]
+    for fn in ("kiwi_ss_size", "kiwi_ss_close"):
+        getattr(lib, fn).argtypes = [C.c_void_p]
+    for fn in ("kiwi_ss_begin_position", "kiwi_ss_end_position"):
+        getattr(lib, fn).argtypes = [C.c_void_p, C.c_int]
+    lib.kiwi_b200_split_batch.restype = C.POINTER(_Sents)
+    lib.kiwi_b200_split_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.kiwi_b200_sents_free.argtypes = [C.POINTER(_Sents)]
     _lib = lib
     return lib
 
@@ -220,14 +237,14 @@ def encode_batch(texts: Sequence[str]) -> Tuple[np.ndarray, np.ndarray]:
 
 
 class _BatchOwner:
-    """keeps the C-side batch (kiwi_b200_batch_t) alive while numpy views of its arrays are in use"""
-    def __init__(self, lib, p):
-        self.lib, self.p = lib, p
+    """keeps the C-side batch (kiwi_b200_batch_t / kiwi_b200_sents_t) alive while numpy views of its arrays are in use"""
+    def __init__(self, lib, p, free="kiwi_b200_batch_free"):
+        self.lib, self.p, self.free = lib, p, free
 
     def __del__(self):
         try:
             if self.p:
-                self.lib.kiwi_b200_batch_free(self.p); self.p = None
+                getattr(self.lib, self.free)(self.p); self.p = None
         except Exception:
             pass
 
@@ -243,6 +260,22 @@ class BatchResult:
 
     def sentence(self, i: int) -> np.ndarray:
         return self.tokens[self.token_offsets[i]:self.token_offsets[i + 1]]
+
+
+@dataclass
+class SentsResult:
+    """kiwi_b200_split_batch: the sentence ranges of every document, [begin, end) in UTF-16 units relative to the document"""
+    sent_offsets: np.ndarray       # uint32 [n + 1] into begin / end
+    begin: np.ndarray              # uint32
+    end: np.ndarray                # uint32
+    status: np.ndarray             # uint32 [n]: 0 = analysed; non-zero = the document exceeded even the escalated device capacity (no ranges)
+    timings_ms: dict
+    _owner: object = None          # the arrays above are views into the library's result buffers (no copy)
+
+    def ranges(self, i: int) -> np.ndarray:
+        """(k, 2) array of document i's sentence ranges"""
+        a, b = int(self.sent_offsets[i]), int(self.sent_offsets[i + 1])
+        return np.stack([self.begin[a:b], self.end[a:b]], axis=1)
 
 
 class Kiwi:
@@ -317,6 +350,49 @@ class Kiwi:
             toks = [(int(k["morph_id"]), tag_to_string(int(k["tag"])), int(k["position"]), int(k["length"]), float(k["score"])) for k in r.sentence(i)]
             out.append([(toks, float(r.scores[i]))])
         return out[0] if single else out
+
+    def split_into_sents(self, text: str, match_options: int = MATCH_ALL_WITH_NORMALIZING, return_tokens: bool = False):
+        """Kiwi::splitIntoSents: [(begin, end), ...] in UTF-16 units of `text`; with return_tokens, (ranges, tokens) where tokens is what
+        analyze(text) returns for the same call (the analysis the ranges come from)."""
+        u = np.ascontiguousarray(np.frombuffer((text + "\0").encode("utf-16-le", "surrogatepass"), dtype="<u2"))
+        res = C.c_void_p(None)
+        ss = self._lib.kiwi_split_into_sents_w(self._h, u.ctypes.data, int(match_options), C.byref(res) if return_tokens else None)
+        if not ss:
+            raise KiwiError(_last_error(self._lib))
+        try:
+            ranges = [(self._lib.kiwi_ss_begin_position(ss, i), self._lib.kiwi_ss_end_position(ss, i)) for i in range(self._lib.kiwi_ss_size(ss))]
+        finally:
+            self._lib.kiwi_ss_close(ss)
+        if not return_tokens:
+            return ranges
+        try:
+            lib, r = self._lib, res.value
+            toks = [(lib.kiwi_res_morpheme_id(r, 0, k, None), lib.kiwi_res_tag(r, 0, k).decode("ascii"), lib.kiwi_res_position(r, 0, k),
+                     lib.kiwi_res_length(r, 0, k), float(lib.kiwi_res_score(r, 0, k))) for k in range(lib.kiwi_res_word_num(r, 0))]
+            return ranges, [(toks, float(lib.kiwi_res_prob(r, 0)))]
+        finally:
+            self._lib.kiwi_res_close(res.value)
+
+    def split_batch(self, texts, match_options: int = MATCH_ALL_WITH_NORMALIZING) -> SentsResult:
+        """kiwi_b200_split_batch over a list of documents or a (UTF-16 blob, offsets[n + 1]) pair"""
+        if isinstance(texts, tuple):
+            blob, offsets = texts
+        else:
+            blob, offsets = encode_batch(texts)
+        blob = np.ascontiguousarray(blob, dtype="<u2"); offsets = np.ascontiguousarray(offsets, dtype=np.uint32)
+        n = len(offsets) - 1
+        p = self._lib.kiwi_b200_split_batch(self._h, blob.ctypes.data, offsets.ctypes.data, n, int(match_options))
+        if not p:
+            raise KiwiError(_last_error(self._lib))
+        owner = _BatchOwner(self._lib, p, "kiwi_b200_sents_free")
+        b = p.contents
+        off = np.ctypeslib.as_array(b.sent_offsets, shape=(n + 1,))
+        total = int(off[n])
+        begin = np.ctypeslib.as_array(b.begin, shape=(total,)) if total else np.zeros(0, np.uint32)
+        end = np.ctypeslib.as_array(b.end, shape=(total,)) if total else np.zeros(0, np.uint32)
+        status = np.ctypeslib.as_array(b.status, shape=(n,)) if n else np.zeros(0, np.uint32)
+        tm = dict(h2d=b.ms_h2d, lattice=b.ms_lattice, viterbi=b.ms_viterbi, sents=b.ms_sents, d2h=b.ms_d2h, total=b.ms_total)
+        return SentsResult(off, begin, end, status, tm, owner)
 
     def analyze_device(self, d_text_ptr: int, d_offsets_ptr: int, n: int, total_units: int, option: AnalyzeOption = None):
         """Inputs already resident in device memory (raw pointers); returns (elapsed_ms, n_tokens, launches)."""

@@ -1,14 +1,17 @@
 // kiwi_b200: host-side result assembly — the token-list post-processing the reference runs after the hot path
 // (SURVEY.md 8f-1).  Pure functions over the finished token list; nothing here touches the device.
-//   fillPairedTokenInfo   /root/reference/src/Kiwi.cpp:98-143   (getSSType src/Utils.cpp:184-261, getSBType 263-298)
-//   SentenceParser        src/Kiwi.cpp:145-290
-//   fillSentLineInfo      src/Kiwi.cpp:322-415   (hasSentences / isNestedLeft / isNestedRight 292-313)
+//   fillPairedTokenInfo   /root/reference/src/Kiwi.cpp:98-143
+//   fillSentLineInfo      src/Kiwi.cpp:322-415
 //   allNewLinePositions   src/Kiwi.cpp:69-96
+// The sentence rules themselves live in sentences.h, which the device sentence kernel (sents.cu) shares; the functions here
+// convert the host's token records to its POD tokens and back.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <string>
 #include <vector>
 #include "kb_model.h"
+#include "sentences.h"
 
 namespace kb
 {
@@ -24,45 +27,6 @@ namespace kb
 		uint32_t sentPosition = 0, lineNumber = 0, subSentPosition = 0, pairedToken = 0xFFFFFFFFu;
 		uint32_t endPos() const { return position + length; }
 	};
-
-	// bracket / quote family of an opening or closing character, 0 = none
-	inline uint32_t ssTypeOf(char16_t c)
-	{
-		static const struct { char16_t open, close; } fam[] = {
-			{ u'\'', u'\'' }, { u'"', u'"' }, { u'(', u')' }, { u'<', u'>' }, { u'[', u']' }, { u'{', u'}' },
-			{ 0x2018, 0x2019 }, { 0x201c, 0x201d }, { 0x226a, 0x226b }, { 0x3008, 0x3009 }, { 0x300a, 0x300b }, { 0x300c, 0x300d },
-			{ 0x300e, 0x300f }, { 0x3010, 0x3011 }, { 0x3014, 0x3015 }, { 0x3016, 0x3017 }, { 0x3018, 0x3019 }, { 0x301a, 0x301b },
-			{ 0xff08, 0xff09 }, { 0xff1c, 0xff1e }, { 0xff3b, 0xff3d }, { 0xff5b, 0xff5d }, { 0xff5f, 0xff60 }, { 0xff62, 0xff63 },
-		};
-		for (uint32_t i = 0; i < sizeof(fam) / sizeof(fam[0]); ++i) if (c == fam[i].open || c == fam[i].close) return i + 1;
-		return 0;
-	}
-
-	// bullet family of an SB token's surface form
-	inline uint32_t sbTypeOf(const std::u16string& form)
-	{
-		if (form.empty()) return 0;
-		uint32_t format = 0, group = 0;
-		uint32_t chr = form[0];
-		if (form.back() == u'.') format = 1;
-		else if (form.back() == u')')
-		{
-			if (form[0] == u'(') { chr = form.size() > 1 ? form[1] : 0; format = 2; }
-			else format = 3;
-		}
-		if (0xAC00 <= chr && chr <= 0xD7A3) group = 1;
-		else if (0x3131 <= chr && chr <= 0x314E) group = 2;
-		else if (u'0' <= chr && chr <= u'9') group = 3;
-		else if (0x2160 <= chr && chr <= 0x216B) group = 4;
-		else if (0x2170 <= chr && chr <= 0x217B) group = 5;
-		else if (0x2460 <= chr && chr <= 0x2473) return 24;
-		else if (0x2780 <= chr && chr <= 0x2789) return 24;
-		else if (0x2776 <= chr && chr <= 0x277F) return 25;
-		else if (0x278A <= chr && chr <= 0x2793) return 25;
-		else if (0x2474 <= chr && chr <= 0x2487) return 26;
-		else if (0x2488 <= chr && chr <= 0x249B) return 27;
-		return format | (group << 2);
-	}
 
 	// ---- surface form of a token that keeps its own substring (TokenInfo::str = joinHangul(PathNode::str), src/Kiwi.cpp:721):
 	// the substring is taken from the NORMALISED text (normalizeHangulWithPosition src/StrUtils.h:493-520, then normalizeCoda
@@ -147,195 +111,43 @@ namespace kb
 	inline std::vector<size_t> newlinePositions(const uint16_t* text, size_t n)
 	{
 		std::vector<size_t> ret;
-		bool afterCR = false;
-		for (size_t i = 0; i < n; ++i)
-		{
-			const uint16_t c = text[i];
-			if (c == 0x0D) { afterCR = true; ret.push_back(i); }
-			else if (c == 0x0A) { if (!afterCR) ret.push_back(i); afterCR = false; }
-			else if (c == 0x0B || c == 0x0C || c == 0x85 || c == 0x2028 || c == 0x2029) { afterCR = false; ret.push_back(i); }
-			else afterCR = false;
-		}
+		for (size_t i = 0; i < n; ++i) if (isNewlineAt(text, (uint32_t)i)) ret.push_back(i);
 		return ret;
+	}
+
+	inline std::vector<SentTok> toSentToks(const std::vector<AsmTok>& toks)
+	{
+		std::vector<SentTok> st(toks.size());
+		for (size_t i = 0; i < toks.size(); ++i)
+		{
+			const AsmTok& t = toks[i];
+			SentTok& o = st[i];
+			o = SentTok{};
+			o.position = t.position; o.length = t.length; o.tag = t.tag; o.flags = t.kformIsYo ? SF_YO : 0;
+			o.wordPosition = t.wordPosition; o.pairedToken = t.pairedToken;
+			setSentForm(o, reinterpret_cast<const uint16_t*>(t.form.data()), (uint32_t)t.form.size());
+		}
+		return st;
 	}
 
 	inline void fillPaired(std::vector<AsmTok>& toks)
 	{
-		std::vector<std::pair<uint32_t, uint32_t>> quotes, bullets;      // (token index, family)
-		for (uint32_t i = 0; i < toks.size(); ++i)
-		{
-			AsmTok& t = toks[i];
-			if (t.tag == T_sso)
-			{
-				const uint32_t type = t.form.empty() ? 0 : ssTypeOf(t.form[0]);
-				if (type) quotes.emplace_back(i, type);
-			}
-			else if (t.tag == T_ssc)
-			{
-				const uint32_t type = t.form.empty() ? 0 : ssTypeOf(t.form[0]);
-				if (!type) continue;
-				for (size_t j = quotes.size(); j-- > 0;)
-				{
-					if (quotes[j].second != type) continue;
-					t.pairedToken = quotes[j].first;
-					toks[quotes[j].first].pairedToken = i;
-					quotes.resize(j);
-					break;
-				}
-			}
-			else if (t.tag == T_sb)
-			{
-				const uint32_t type = sbTypeOf(t.form);
-				if (!type) continue;
-				for (size_t j = bullets.size(); j-- > 0;)
-				{
-					if (bullets[j].second != type) continue;
-					toks[bullets[j].first].pairedToken = i;
-					bullets.resize(j);
-					break;
-				}
-				bullets.emplace_back(i, type);
-			}
-		}
+		std::vector<SentTok> st = toSentToks(toks);
+		std::vector<uint2> stacks(2 * st.size() + 2);
+		pairTokens(st.data(), (uint32_t)st.size(), stacks.data(), stacks.data() + st.size() + 1);
+		for (size_t i = 0; i < toks.size(); ++i) toks[i].pairedToken = st[i].pairedToken;
 	}
 
-	// sentence boundary automaton: a sentence ends after a final ending (+ optional "요", z_coda) or final punctuation,
-	// followed by any run of closing symbols; see the rule comment at src/Kiwi.cpp:145-150
-	class SentenceSplitter
-	{
-		enum { S_none, S_ef, S_efjx, S_zcoda, S_sf } state = S_none;
-		size_t lastPosition = 0, lastLineNumber = 0;
-		static bool trailingSymbol(uint8_t tag) { return tag == T_so || tag == T_sw || tag == T_sh || tag == T_sp || tag == T_se || tag == T_ssc; }
-	public:
-		bool next(const AsmTok& t, size_t lineNumber, bool forceNewSent = false)
-		{
-			bool ret = false;
-			if (forceNewSent)
-			{
-				state = S_none;
-				lastPosition = t.position + t.length;
-				return true;
-			}
-			const uint8_t tag = t.tag;
-			if (state == S_none)
-			{
-				if (tag == T_ef) state = S_ef;
-				else if (tag == T_sf) state = S_sf;
-			}
-			else if (state == S_ef || state == S_efjx)
-			{
-				if (state == S_ef && tag == T_vx) state = S_none;
-				else if (tag == T_z_coda) state = S_zcoda;
-				else if (isJClass(tag) || tag == T_vcp || tag == T_etm || tag == T_ec)
-				{
-					if (tag == T_jx && t.kformIsYo)
-					{
-						if (state == S_ef) state = S_efjx;
-						else { ret = true; state = S_none; }
-					}
-					else state = S_none;
-				}
-				else if (trailingSymbol(tag)) {}
-				else if (tag == T_sf) state = S_sf;
-				else if (tag == T_sso && lineNumber == lastLineNumber) {}
-				else { ret = true; state = S_none; }
-			}
-			else if (state == S_zcoda)
-			{
-				if (trailingSymbol(tag) || tag == T_sf) {}
-				else if (tag == T_sso && lineNumber == lastLineNumber) {}
-				else { ret = true; state = S_none; }
-			}
-			else      // S_sf
-			{
-				if (trailingSymbol(tag)) {}
-				else if (tag == T_sso)
-				{
-					if (lineNumber != lastLineNumber) { ret = true; state = S_none; }
-				}
-				else if ((tag == T_sl || tag == T_sn) && lastPosition == t.position) state = S_none;
-				else { ret = true; state = S_none; }
-			}
-			lastPosition = t.position + t.length;
-			lastLineNumber = lineNumber;
-			return ret;
-		}
-	};
-
-	inline bool hasSentences(const AsmTok* first, const AsmTok* last)
-	{
-		SentenceSplitter sp;
-		for (; first != last; ++first) if (sp.next(*first, 0)) return true;
-		return sp.next(AsmTok{}, 0);
-	}
-	inline bool isNestedLeft(const AsmTok& t) { return isJClass(t.tag) || (isEClass(t.tag) && t.tag != T_ef) || t.tag == T_sp; }
-	inline bool isNestedRight(const AsmTok& t)
-	{
-		return isJClass(t.tag) || isEClass(t.tag) || (isVerbClass(t.tag) && t.form.size() == 1 && t.form[0] == 0xD558) || t.tag == T_vcp || t.tag == T_sp;
-	}
-
+	// (pairedToken filled by fillPaired)
 	inline void fillSentLine(std::vector<AsmTok>& toks, const std::vector<size_t>& newlines)
 	{
-		SentenceSplitter sp;
-		uint32_t sentPos = 0, lastSentPos = 0, subSentPos = 0, accumSubSent = 1, accumWordPos = 0, lastWordPos = 0;
-		size_t nlPos = 0, lastNlPos = 0, nestedSentEnd = 0, nestedEnd = 0;
+		std::vector<SentTok> st = toSentToks(toks);
+		for (auto& t : st) t.lineNumber = (uint32_t)(std::lower_bound(newlines.begin(), newlines.end(), (size_t)t.position) - newlines.begin());
+		foldSentLine(st.data(), (uint32_t)st.size());
 		for (size_t i = 0; i < toks.size(); ++i)
 		{
 			AsmTok& t = toks[i];
-			if (i >= nestedEnd && sp.next(t, nlPos, nestedSentEnd && i == nestedSentEnd))
-			{
-				const bool includePrevToken = i > 1
-					&& (toks[i - 1].tag == T_so || toks[i - 1].tag == T_sw || toks[i - 1].tag == T_sp || toks[i - 1].tag == T_se || toks[i - 1].tag == T_sso)
-					&& toks[i - 1].endPos() == toks[i].position
-					&& toks[i - 1].position > toks[i - 2].endPos();
-				if (nestedSentEnd)
-				{
-					subSentPos++;
-					accumSubSent++;
-					if (includePrevToken) toks[i - 1].subSentPosition = subSentPos;
-				}
-				else
-				{
-					sentPos++;
-					accumSubSent = 1;
-					if (includePrevToken)
-					{
-						toks[i - 1].sentPosition = sentPos;
-						toks[i - 1].wordPosition = 0;
-						accumWordPos = 0;
-					}
-				}
-			}
-
-			if (!nestedSentEnd && !nestedEnd && t.tag == T_sso && t.pairedToken != 0xFFFFFFFFu)
-			{
-				if (!hasSentences(&toks[i], &toks[t.pairedToken]))
-				{
-					nestedEnd = t.pairedToken;
-					subSentPos = 0;
-				}
-				else if ((t.pairedToken + 1 < toks.size() && isNestedRight(toks[t.pairedToken + 1])) || (i > 0 && isNestedLeft(toks[i - 1])))
-				{
-					nestedSentEnd = t.pairedToken;
-					subSentPos = accumSubSent;
-				}
-			}
-			else if (nestedSentEnd && i > nestedSentEnd) { nestedSentEnd = 0; subSentPos = 0; }
-			else if (nestedEnd && i >= nestedEnd) { nestedEnd = 0; subSentPos = 0; }
-
-			while (nlPos < newlines.size() && newlines[nlPos] < t.position) nlPos++;
-			t.lineNumber = (uint32_t)nlPos;
-			if (nlPos > lastNlPos + 1 && sentPos == lastSentPos && !nestedSentEnd) sentPos++;
-			t.sentPosition = sentPos;
-			t.subSentPosition = (i == nestedSentEnd || i == toks[nestedSentEnd].pairedToken) ? 0 : subSentPos;
-
-			if (sentPos != lastSentPos) { accumWordPos = 0; accumSubSent = 1; }
-			else if (t.wordPosition != lastWordPos) accumWordPos++;
-			lastWordPos = t.wordPosition;
-			t.wordPosition = accumWordPos;
-
-			lastSentPos = sentPos;
-			lastNlPos = nlPos;
+			t.wordPosition = st[i].wordPosition; t.sentPosition = st[i].sentPosition; t.lineNumber = st[i].lineNumber; t.subSentPosition = st[i].subSentPosition;
 		}
 	}
 }

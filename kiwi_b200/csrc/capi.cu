@@ -95,6 +95,8 @@ struct BlockScope      // AnalyzeOption::blocklist for the calls made while the 
 	~BlockScope() { e->setCandsOverride(nullptr); }
 };
 
+struct kiwi_ss { std::vector<std::pair<uint32_t, uint32_t>> ranges; };      // capi/kiwi_c.cpp: kiwi_ss = vector<pair<size_t, size_t>>
+
 struct kiwi_res
 {
 	struct Tok { kiwi_token_info_t info; uint32_t morphId; std::u16string form; std::string form8; };
@@ -130,7 +132,8 @@ static const char16_t* tagNameW(uint8_t t)
 	return b.c_str();
 }
 
-static std::u16string utf8To16(const char* s)
+// bytePositions (optional): the byte offset of the character every UTF-16 unit belongs to, + the length (utf8To16, src/StrUtils.h:236-300)
+static std::u16string utf8To16(const char* s, std::vector<uint32_t>* bytePositions = nullptr)
 {
 	std::u16string out;
 	const size_t n = std::strlen(s);
@@ -139,10 +142,12 @@ static std::u16string utf8To16(const char* s)
 		uint32_t c = (uint8_t)s[i]; size_t k = 1;
 		if (c >= 0xF0) { c &= 7; k = 4; } else if (c >= 0xE0) { c &= 15; k = 3; } else if (c >= 0xC0) { c &= 31; k = 2; }
 		for (size_t j = 1; j < k && i + j < n; ++j) c = (c << 6) | ((uint8_t)s[i + j] & 63);
+		if (bytePositions) bytePositions->insert(bytePositions->end(), c >= 0x10000 ? 2 : 1, (uint32_t)i);
 		i += k;
 		if (c >= 0x10000) { c -= 0x10000; out.push_back((char16_t)(0xD800 | (c >> 10))); out.push_back((char16_t)(0xDC00 | (c & 0x3FF))); }
 		else out.push_back((char16_t)c);
 	}
+	if (bytePositions) bytePositions->push_back((uint32_t)n);
 	return out;
 }
 static std::string utf16To8(const std::u16string& s)
@@ -240,14 +245,16 @@ static kiwi_res* makeRes(kiwi_s* h, const uint16_t* text, uint32_t rawLen, const
 // One batch through the handle's engine(s).  With several devices (kiwi_b200_init_multi) sentence i goes to device i mod N
 // (BASELINE.json config 5); one host thread per device gathers its shard, runs it, and scatters its rows back into the batch's
 // output arrays in input order - the reference's ordered delivery (include/kiwi/Kiwi.h:402-454) without a collective.
-static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offsets, uint32_t n, const kiwi_analyze_option_t& option, BatchOutput& out)
+// `outputs` (OUT_*): the token rows and / or the sentence ranges (kiwi_split_into_sents, kiwi_b200_split_batch), merged alike.
+static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offsets, uint32_t n, const kiwi_analyze_option_t& option, BatchOutput& out,
+	uint32_t outputs = OUT_TOKENS)
 {
 	const uint32_t N = 1 + (uint32_t)h->extra.size();
 	if (N == 1 || n < 2 * N)
 	{
 		TypoScope ts{ h->engine.get(), option };
 		BlockScope bs{ h->engine.get(), option };
-		h->engine->analyze(text, offsets, n, optionWord(option), out);
+		h->engine->analyze(text, offsets, n, optionWord(option), out, outputs);
 		return;
 	}
 	if (h->shardOut.size() != N) h->shardOut.resize(N);
@@ -272,7 +279,7 @@ static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offs
 			const auto t1 = Clock::now();
 			TypoScope ts{ e, option };
 			BlockScope bs{ e, option };
-			e->analyze(sub.data(), off.data(), (uint32_t)off.size() - 1, optionWord(option), part[r]);
+			e->analyze(sub.data(), off.data(), (uint32_t)off.size() - 1, optionWord(option), part[r], outputs);
 			stats[r] = e->last;
 			msGather[r] = std::chrono::duration<double, std::milli>(t1 - t0).count();
 			msEngine[r] = std::chrono::duration<double, std::milli>(Clock::now() - t1).count();
@@ -287,16 +294,20 @@ static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offs
 	// ordered merge: token offsets by prefix sum over the round-robin order, then every shard scatters its rows
 	// (`out` may be a recycled holder: its arrays keep their capacity)
 	const auto tMerge = Clock::now();
-	out.msH2D = out.msLattice = out.msViterbi = out.msPack = out.msD2H = out.msTotal = 0;
+	out.msH2D = out.msLattice = out.msViterbi = out.msPack = out.msSents = out.msD2H = out.msTotal = 0;
 	out.tokens.clear();
 	out.tokOff.assign((size_t)n + 1, 0); out.scores.resize(n); out.status.resize(n);
+	const bool sents = (outputs & OUT_SENTS) != 0;
+	out.sentOff.assign(sents ? (size_t)n + 1 : 0, 0);
 	for (uint32_t i = 0; i < n; ++i)
 	{
 		const BatchOutput& p = part[i % N]; const uint32_t k = i / N;
 		out.tokOff[i + 1] = out.tokOff[i] + (p.tokOff[k + 1] - p.tokOff[k]);
 		out.scores[i] = p.scores[k]; out.status[i] = p.status[k];
+		if (sents) out.sentOff[i + 1] = out.sentOff[i] + (p.sentOff[k + 1] - p.sentOff[k]);
 	}
 	out.tokens.resize(out.tokOff[n]);
+	out.sentBegin.resize(sents ? out.sentOff[n] : 0); out.sentEnd.resize(sents ? out.sentOff[n] : 0);
 	auto scatter = [&](uint32_t r)
 	{
 		const BatchOutput& p = part[r];
@@ -304,6 +315,10 @@ static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offs
 		{
 			const uint32_t cnt = p.tokOff[k + 1] - p.tokOff[k];
 			if (cnt) std::memcpy(out.tokens.data() + out.tokOff[i], p.tokens.data() + p.tokOff[k], (size_t)cnt * sizeof(DToken));
+			if (!sents) continue;
+			const uint32_t ns = p.sentOff[k + 1] - p.sentOff[k];
+			std::copy_n(p.sentBegin.data() + p.sentOff[k], ns, out.sentBegin.data() + out.sentOff[i]);
+			std::copy_n(p.sentEnd.data() + p.sentOff[k], ns, out.sentEnd.data() + out.sentOff[i]);
 		}
 	};
 	th.clear();
@@ -315,7 +330,7 @@ static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offs
 	{
 		const BatchOutput& p = part[r];
 		out.msH2D = std::max(out.msH2D, p.msH2D); out.msLattice = std::max(out.msLattice, p.msLattice); out.msViterbi = std::max(out.msViterbi, p.msViterbi);
-		out.msPack = std::max(out.msPack, p.msPack); out.msD2H = std::max(out.msD2H, p.msD2H); out.msTotal = std::max(out.msTotal, p.msTotal);
+		out.msPack = std::max(out.msPack, p.msPack); out.msSents = std::max(out.msSents, p.msSents); out.msD2H = std::max(out.msD2H, p.msD2H); out.msTotal = std::max(out.msTotal, p.msTotal);
 		agg.h2dBytes += stats[r].h2dBytes; agg.d2hBytes += stats[r].d2hBytes; agg.kernelLaunches += stats[r].kernelLaunches; agg.retried += stats[r].retried;
 		agg.rawUnits += stats[r].rawUnits;
 	}
@@ -717,6 +732,58 @@ float kiwi_res_score(kiwi_res_h result, int index, int num) { KB_TOK_OR(0.f) ret
 float kiwi_res_typo_cost(kiwi_res_h result, int index, int num) { KB_TOK_OR(0.f) return result->toks[num].info.typo_cost; }
 int kiwi_res_close(kiwi_res_h result) { if (!result) return KIWIERR_INVALID_HANDLE; delete result; return 0; }
 
+// ---- sentence splitting (Kiwi::splitIntoSents): one engine call brings the ranges and, for tokenized_res, the token rows ----
+kiwi_ss_h kiwi_split_into_sents_w(kiwi_h handle, const kchar16_t* text, int match_options, kiwi_res_h* tokenized_res)
+{
+	if (!handle) return nullptr;
+	try
+	{
+		kiwi_analyze_option_t option{};
+		option.match_options = match_options;
+		checkOption(option, 1, nullptr);
+		uint32_t len = 0;
+		while (text[len]) ++len;
+		const uint32_t off[2] = { 0, len };
+		std::lock_guard<std::mutex> lk(handle->mtx);
+		BatchOutput& bo = handle->callOut;
+		analyzeSharded(handle, text, off, 1, option, bo, OUT_SENTS | (tokenized_res ? OUT_TOKENS : 0));
+		auto ss = std::make_unique<kiwi_ss>();
+		for (uint32_t k = bo.sentOff[0]; k < bo.sentOff[1]; ++k) ss->ranges.emplace_back(bo.sentBegin[k], bo.sentEnd[k]);
+		if (tokenized_res) *tokenized_res = makeRes(handle, text, len, bo, 0, (uint32_t)match_options);
+		return ss.release();
+	}
+	catch (const std::exception& e) { setError(e); return nullptr; }
+}
+
+kiwi_ss_h kiwi_split_into_sents(kiwi_h handle, const char* text, int match_options, kiwi_res_h* tokenized_res)
+{
+	if (!handle) return nullptr;
+	try
+	{
+		std::vector<uint32_t> bytePositions;
+		const std::u16string w = utf8To16(text, &bytePositions);
+		kiwi_ss_h ss = kiwi_split_into_sents_w(handle, reinterpret_cast<const kchar16_t*>(w.c_str()), match_options, tokenized_res);
+		if (ss) for (auto& r : ss->ranges) { r.first = bytePositions[r.first]; r.second = bytePositions[r.second]; }      // (Kiwi.cpp:438-450)
+		return ss;
+	}
+	catch (const std::exception& e) { setError(e); return nullptr; }
+}
+
+int kiwi_ss_size(kiwi_ss_h result) { if (!result) return KIWIERR_INVALID_HANDLE; return (int)result->ranges.size(); }
+int kiwi_ss_begin_position(kiwi_ss_h result, int index)
+{
+	if (!result) return KIWIERR_INVALID_HANDLE;
+	if (index < 0 || index >= (int)result->ranges.size()) return KIWIERR_INVALID_INDEX;
+	return (int)result->ranges[index].first;
+}
+int kiwi_ss_end_position(kiwi_ss_h result, int index)
+{
+	if (!result) return KIWIERR_INVALID_HANDLE;
+	if (index < 0 || index >= (int)result->ranges.size()) return KIWIERR_INVALID_INDEX;
+	return (int)result->ranges[index].second;
+}
+int kiwi_ss_close(kiwi_ss_h result) { if (!result) return KIWIERR_INVALID_HANDLE; delete result; return 0; }
+
 const kiwi_b200_batch_t* kiwi_b200_analyze_batch(kiwi_h handle, const kchar16_t* text, const uint32_t* offsets, int n, kiwi_analyze_option_t option)
 {
 	if (!handle) { setError("invalid handle"); return nullptr; }
@@ -749,6 +816,36 @@ const kiwi_b200_batch_t* kiwi_b200_analyze_batch(kiwi_h handle, const kchar16_t*
 		return &h->pub;
 	}
 	catch (const std::exception& e) { setError(e); return nullptr; }
+}
+
+struct SentsHolder { kiwi_b200_sents_t pub; BatchOutput bo; };
+
+const kiwi_b200_sents_t* kiwi_b200_split_batch(kiwi_h handle, const kchar16_t* text, const uint32_t* offsets, int n, int match_options)
+{
+	if (!handle) { setError("invalid handle"); return nullptr; }
+	try
+	{
+		kiwi_analyze_option_t option{};
+		option.match_options = match_options;
+		checkOption(option, 1, nullptr);
+		if (n < 0) throw std::invalid_argument("n < 0");
+		auto h = std::make_unique<SentsHolder>();
+		{
+			std::lock_guard<std::mutex> lk(handle->mtx);
+			analyzeSharded(handle, text, offsets, (uint32_t)n, option, h->bo, OUT_SENTS);
+		}
+		h->pub.n_docs = n;
+		h->pub.sent_offsets = h->bo.sentOff.data(); h->pub.begin = h->bo.sentBegin.data(); h->pub.end = h->bo.sentEnd.data(); h->pub.status = h->bo.status.data();
+		h->pub.ms_h2d = h->bo.msH2D; h->pub.ms_lattice = h->bo.msLattice; h->pub.ms_viterbi = h->bo.msViterbi; h->pub.ms_sents = h->bo.msSents;
+		h->pub.ms_d2h = h->bo.msD2H; h->pub.ms_total = h->bo.msTotal;
+		return &h.release()->pub;
+	}
+	catch (const std::exception& e) { setError(e); return nullptr; }
+}
+
+void kiwi_b200_sents_free(const kiwi_b200_sents_t* sents)
+{
+	delete reinterpret_cast<SentsHolder*>(const_cast<kiwi_b200_sents_t*>(sents));
 }
 
 void kiwi_b200_batch_free(const kiwi_b200_batch_t* batch)

@@ -35,6 +35,9 @@ namespace kb
 	cudaError_t launch_cong_debug(uint32_t n, const uint32_t* ctx, const uint32_t* wid, const int32_t* node,
 		int32_t* outDot, float* outEps, int32_t* outNode, uint32_t* outCtx, int32_t* outTile, cudaStream_t stream);
 	cudaError_t set_model_emit(const DevModel& m);
+	cudaError_t launch_sents(const BatchView& bv, const VitView& vv, uint32_t* nSents, cudaStream_t stream);
+	cudaError_t launch_sents_pack(const BatchView& bv, const uint32_t* nSents, const uint32_t* sentOff, uint32_t* begin, uint32_t* end, cudaStream_t stream);
+	cudaError_t set_model_sents(const DevModel& m);
 
 	static void ck(cudaError_t e, const char* what)
 	{
@@ -108,7 +111,8 @@ namespace kb
 	// ---- per-device state: one lock and one owner of the kernels' __constant__ model view per CUDA device --------------
 	namespace
 	{
-		struct DevState { std::recursive_mutex mtx; const Model* owner = nullptr; };
+		// (sentsOwner: the model view of the sentence kernel, uploaded by the first split only)
+		struct DevState { std::recursive_mutex mtx; const Model* owner = nullptr; const Model* sentsOwner = nullptr; };
 		DevState g_devState[64];
 	}
 	DeviceGuard::DeviceGuard(int device) : dev{ device < 0 || device >= 64 ? 0 : device }
@@ -134,6 +138,7 @@ namespace kb
 		{
 			ck(cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking), "cudaStreamCreate");
 			for (auto& e : sl.ev) ck(cudaEventCreate(&e), "cudaEventCreate");
+			for (auto& e : sl.evSents) ck(cudaEventCreate(&e), "cudaEventCreate");
 		}
 		stream = slot_[0].stream;
 	}
@@ -142,6 +147,7 @@ namespace kb
 	{
 		DeviceGuard g{ device };
 		if (g_devState[g.dev].owner == &model) g_devState[g.dev].owner = nullptr;
+		if (g_devState[g.dev].sentsOwner == &model) g_devState[g.dev].sentsOwner = nullptr;
 		for (auto& sl : slot_)
 		{
 			freeScratch(sl.sc);
@@ -149,6 +155,7 @@ namespace kb
 			if (sl.hPinOff) cudaFreeHost(sl.hPinOff);
 			if (sl.hPinOut) cudaFreeHost(sl.hPinOut);
 			for (auto& e : sl.ev) if (e) cudaEventDestroy(e);
+			for (auto& e : sl.evSents) if (e) cudaEventDestroy(e);
 			if (sl.stream) cudaStreamDestroy(sl.stream);
 		}
 		freeScratch(retry_);
@@ -158,6 +165,7 @@ namespace kb
 	{
 		for (void* p : sc.bufs) cudaFree(p);
 		for (void* p : sc.typoBufs) cudaFree(p);
+		for (void* p : sc.sentBufs) cudaFree(p);
 		sc = Scratch{};
 	}
 
@@ -342,6 +350,55 @@ namespace kb
 		return t;
 	}
 
+	// ---- sentence ranges (Kiwi::splitIntoSents): sents_kernel over the unpacked token rows, then a scan and a pack like the tokens' ----
+	void Engine::ensureSentScratch(Scratch& sc)
+	{
+		if (sc.sentCapUnits >= sc.capUnits && sc.sentCapSent >= sc.capSent) return;
+		for (void* p : sc.sentBufs) cudaFree(p);
+		sc.sentBufs.clear();
+		auto alloc = [&](size_t bytes) { void* p = nullptr; ck(cudaMalloc(&p, std::max<size_t>(bytes, 256)), "cudaMalloc(sentence scratch)"); sc.sentBufs.push_back(p); return (uint32_t*)p; };
+		// (a document has at most as many sentences as tokens, and at most W_s tokens: the packed ranges fit capUnits)
+		sc.nSents = alloc((sc.capSent + 1) * 4); sc.sentOff = alloc((sc.capSent + 1) * 4);
+		sc.sentBegin = alloc(sc.capUnits * 4); sc.sentEnd = alloc(sc.capUnits * 4);
+		sc.sentCapUnits = sc.capUnits; sc.sentCapSent = sc.capSent;
+	}
+
+	// after launchAll on the same stream (ensureSentScratch first)
+	void Engine::launchSents(Scratch& sc, cudaStream_t st, cudaEvent_t* evSents, uint32_t n)
+	{
+		DevState& ds = g_devState[device < 0 || device >= 64 ? 0 : device];
+		if (ds.sentsOwner != &model) { ck(set_model_sents(model.dev), "constant upload"); ds.sentsOwner = &model; }
+		ck(cudaEventRecord(evSents[0], st), "event");
+		ck(launch_sents(sc.bv, sc.vv, sc.nSents, st), "sents_kernel launch");
+		ck(cudaMemsetAsync(sc.nSents + n, 0, 4, st), "memset");
+		size_t tb = sc.cubTempBytes;
+		ck(cub::DeviceScan::ExclusiveSum(sc.cubTemp, tb, sc.nSents, sc.sentOff, (int)(n + 1), st), "cub scan");
+		ck(launch_sents_pack(sc.bv, sc.nSents, sc.sentOff, sc.sentBegin, sc.sentEnd, st), "sents_pack_kernel launch");
+		ck(cudaEventRecord(evSents[1], st), "event");
+		last.kernelLaunches += 3;
+	}
+
+	// appends the ranges of the n sentences of a finished launch (hSentOff: its sentOff scan, on the host) to `out`; its kernel time counts
+	// as msSents, the copy as D2H
+	void Engine::copySents(Scratch& sc, cudaStream_t st, cudaEvent_t* evSents, uint32_t n, const uint32_t* hSentOff, BatchOutput& out)
+	{
+		const size_t base = out.sentBegin.size(), total = hSentOff[n];
+		out.sentBegin.resize(base + total); out.sentEnd.resize(base + total);
+		ck(cudaEventRecord(evSents[2], st), "event");
+		if (total)
+		{
+			ck(cudaMemcpyAsync(out.sentBegin.data() + base, sc.sentBegin, total * 4, cudaMemcpyDeviceToHost, st), "D2H sentence ranges");
+			ck(cudaMemcpyAsync(out.sentEnd.data() + base, sc.sentEnd, total * 4, cudaMemcpyDeviceToHost, st), "D2H sentence ranges");
+		}
+		ck(cudaEventRecord(evSents[3], st), "event");
+		ck(cudaEventSynchronize(evSents[3]), "sync (sentence ranges)");
+		for (uint32_t k = 1; k <= n; ++k) out.sentOff.push_back((uint32_t)(base + hSentOff[k]));
+		float ms = 0;
+		cudaEventElapsedTime(&ms, evSents[0], evSents[1]); out.msSents += ms;
+		cudaEventElapsedTime(&ms, evSents[2], evSents[3]); out.msD2H += ms; out.msTotal += ms;
+		last.d2hBytes += total * 8;
+	}
+
 	// KIWI_B200_SOLO=<blocks>,<warps> (work-queue kernel build): the first <blocks> blocks of the Viterbi wave keep only <warps> warps,
 	// which start with the heaviest sentences of the launch order
 	static std::pair<uint32_t, uint32_t> soloConfig()
@@ -384,7 +441,7 @@ namespace kb
 		}
 	}
 
-	// Layout of a slot's pinned head buffer: [tokOff n+1][scores n][status n][debug flag 2 words].  The packed tokens go straight into
+	// Layout of a slot's pinned head buffer: [tokOff n+1][scores n][status n][debug flag 2 words], + [sentOff n+1] with OUT_SENTS.  The packed tokens go straight into
 	// the caller's (page-locked) result array:
 	//  - the FIRST pass of a call knows where its tokens start (offset 0), so an ESTIMATE of them (5/8 token per raw UTF-16 unit + 8 per
 	//    sentence; web text needs ~0.55) is enqueued behind the kernels together with the head - a single-pass call needs one stream
@@ -410,7 +467,7 @@ namespace kb
 	// a sentence that overflowed an arena may fit a larger one; a chunk beyond the 16-bit node index (ST_TOO_LONG) fits none
 	static bool retryable(uint32_t status) { return status && status != ST_TOO_LONG; }
 
-	void Engine::submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t pn, uint32_t matchOptions, DToken* directDst)
+	void Engine::submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t pn, uint32_t matchOptions, DToken* directDst, uint32_t outputs)
 	{
 		const size_t t0 = off[i0], pT = off[i0 + pn] - t0;
 		const size_t U = 2 * pT + 4 * (size_t)pn;
@@ -423,8 +480,11 @@ namespace kb
 		ck(cudaMemcpyAsync(s.sc.dText, s.hPinText, pT * 2, cudaMemcpyHostToDevice, s.stream), "H2D text");
 		ck(cudaMemcpyAsync(s.sc.dOff, s.hPinOff, ((size_t)pn + 1) * 4, cudaMemcpyHostToDevice, s.stream), "H2D offsets");
 		bind(s.sc, s.sc.dText, s.sc.dOff, pn, matchOptions, 1);
+		const bool sents = (outputs & OUT_SENTS) != 0;
+		if (sents) ensureSentScratch(s.sc);
 		launchAll(s.sc, s.stream, s.ev, pn);
-		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2;
+		if (sents) launchSents(s.sc, s.stream, s.evSents, pn);
+		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2 + (sents ? (size_t)pn + 1 : 0);
 		const size_t est = directDst ? std::min(tokenEstimate(pT, pn), (size_t)U) : 0;
 		growPinned(&s.hPinOut, &s.pinOutCap, headWords * 4 + 16);
 		uint32_t* hTokOff = (uint32_t*)s.hPinOut; float* hScore = (float*)(hTokOff + pn + 1); uint32_t* hStatus = (uint32_t*)(hScore + pn); uint32_t* hDbg = hStatus + pn;
@@ -433,6 +493,7 @@ namespace kb
 		ck(cudaMemcpyAsync(hStatus, s.sc.bv.status, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H status");
 		ck(cudaMemcpyAsync(hDbg, s.sc.bv.debug, 4, cudaMemcpyDeviceToHost, s.stream), "D2H debug");
 		ck(cudaMemcpyAsync(hDbg + 1, model.dev.debug, 4, cudaMemcpyDeviceToHost, s.stream), "D2H debug");
+		if (sents) ck(cudaMemcpyAsync(hDbg + 2, s.sc.sentOff, ((size_t)pn + 1) * 4, cudaMemcpyDeviceToHost, s.stream), "D2H sentence offsets");
 		if (est) ck(cudaMemcpyAsync(directDst, s.sc.packed, est * sizeof(DToken), cudaMemcpyDeviceToHost, s.stream), "D2H tokens");
 		ck(cudaEventRecord(s.ev[5], s.stream), "event");
 		s.busy = true; s.n = pn; s.tokCopied = est;
@@ -453,7 +514,7 @@ namespace kb
 	}
 
 	// waits for the slot's pass, appends its sentences (they are the next ones in input order) to `out`
-	void Engine::finishPass(Slot& s, BatchOutput& out)
+	void Engine::finishPass(Slot& s, BatchOutput& out, uint32_t outputs)
 	{
 		if (!s.busy) return;
 		ck(cudaStreamSynchronize(s.stream), "sync (a kernel fault surfaces here)");
@@ -465,10 +526,11 @@ namespace kb
 			cudaEventElapsedTime(&ms, s.ev[6], s.ev[7]); out.msD2H += ms; out.msTotal += ms;
 		}
 		const uint32_t pn = s.n;
-		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2;
+		const bool tokens = (outputs & OUT_TOKENS) != 0, sents = (outputs & OUT_SENTS) != 0;
+		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2 + (sents ? (size_t)pn + 1 : 0);
 		const uint32_t* hTokOff = (const uint32_t*)s.hPinOut; const float* hScore = (const float*)(hTokOff + pn + 1); const uint32_t* hStatus = (const uint32_t*)(hScore + pn); const uint32_t* hDbg = hStatus + pn;
 		if (hDbg[0] || hDbg[1]) checkDebug(s.sc);
-		const uint32_t total = hTokOff[pn];
+		const uint32_t total = tokens ? hTokOff[pn] : 0;
 		const size_t base = out.tokens.size();
 		// what the first pass copied on its own is in place already (base == 0 there); make it part of the array before anything can move it
 		const size_t first = std::min<size_t>(total, s.tokCopied);
@@ -484,7 +546,7 @@ namespace kb
 		}
 		for (uint32_t k = 0; k < pn; ++k)
 		{
-			out.tokOff.push_back((uint32_t)(base + hTokOff[k + 1]));
+			out.tokOff.push_back((uint32_t)(base + (tokens ? hTokOff[k + 1] : 0)));
 			out.scores.push_back(hScore[k]); out.status.push_back(hStatus[k]);
 		}
 		const KernelMs t = kernelMs(s.ev);
@@ -494,6 +556,7 @@ namespace kb
 		cudaEventElapsedTime(&ms, s.ev[4], s.ev[5]); out.msD2H += ms;
 		cudaEventElapsedTime(&ms, s.ev[0], s.ev[5]); out.msTotal += ms;
 		last.d2hBytes += headWords * 4 + (size_t)std::max<size_t>(total, s.tokCopied) * sizeof(DToken);
+		if (sents) copySents(s.sc, s.stream, s.evSents, pn, hDbg + 2, out);
 	}
 
 	// Sentences that overflowed the arithmetic capacity of a main arena are re-run in the retry arena with 8 x the path and 4 x the
@@ -501,27 +564,30 @@ namespace kb
 	// budget.  runRetry runs round `round` and the rounds after it over the n sentences of the contiguous sub-batch text / offsets:
 	// `out.status` holds on entry the status each of them failed with, and `out` receives their results.  A sentence that fails even
 	// then keeps its status and has no tokens: the caller reports it per sentence instead of failing the whole batch.
-	void Engine::runRetry(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, int round, BatchOutput& out)
+	void Engine::runRetry(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, int round, BatchOutput& out, uint32_t outputs)
 	{
+		const bool tokens = (outputs & OUT_TOKENS) != 0, sents = (outputs & OUT_SENTS) != 0;
 		static const uint32_t pathMul[2] = { 8, 64 }, nodeMul[2] = { 4, 16 };
 		const size_t budget = (size_t)4 << 30;       // bytes of path pool per sub-pass (the retry arena stays allocated with its handle)
 		const uint32_t ppu = DEFAULT_PATHS_PER_UNIT * pathScale() * pathMul[round], pc = DEFAULT_PATHS_CONST * pathScale() * pathMul[round], npu = KB_DEFAULT_NODES_PER_UNIT * nodeMul[round];
 		const auto fits = [&](size_t units, size_t count) { return (units * ppu + count * pc) * pathStride() <= budget; };
 		Slot& s = slot_[0];
 		out.tokOff.assign(1, 0); out.tokens.clear(); out.scores.assign(n, 0.f);
-		std::vector<uint32_t> subOff, tokOff;
+		if (sents) { out.sentOff.assign(1, 0); out.sentBegin.clear(); out.sentEnd.clear(); }
+		std::vector<uint32_t> subOff, tokOff, sentOff;
 		for (uint32_t i0 = 0, i1; i0 < n; i0 = i1)
 		{
 			i1 = passEnd(offsets, i0, n, fits);
 			const uint32_t pn = i1 - i0;
 			const size_t t0 = offsets[i0], pT = offsets[i1] - t0, U = 2 * pT + 4 * (size_t)pn;
-			try { ensureScratch(retry_, s.stream, U, pn, ppu, pc, npu); }
+			try { ensureScratch(retry_, s.stream, U, pn, ppu, pc, npu); if (sents) ensureSentScratch(retry_); }
 			catch (const std::exception&)
 			{
 				// the escalated arena does not fit the device: these sentences keep their overflow status (no tokens), the batch goes on
 				cudaGetLastError();
 				freeScratch(retry_);
 				out.tokOff.resize(out.tokOff.size() + pn, (uint32_t)out.tokens.size());
+				if (sents) out.sentOff.resize(out.sentOff.size() + pn, (uint32_t)out.sentBegin.size());
 				continue;
 			}
 			subOff.resize((size_t)pn + 1);
@@ -530,26 +596,36 @@ namespace kb
 			ck(cudaMemcpyAsync(retry_.dOff, subOff.data(), ((size_t)pn + 1) * 4, cudaMemcpyHostToDevice, s.stream), "H2D offsets");
 			bind(retry_, retry_.dText, retry_.dOff, pn, matchOptions, nodeMul[round]);
 			launchAll(retry_, s.stream, s.ev, pn);
+			if (sents) launchSents(retry_, s.stream, s.evSents, pn);
 			tokOff.resize((size_t)pn + 1);
 			ck(cudaMemcpyAsync(tokOff.data(), retry_.tokOff, ((size_t)pn + 1) * 4, cudaMemcpyDeviceToHost, s.stream), "D2H offsets");
 			ck(cudaMemcpyAsync(out.scores.data() + i0, retry_.vv.score, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H scores");
 			ck(cudaMemcpyAsync(out.status.data() + i0, retry_.bv.status, (size_t)pn * 4, cudaMemcpyDeviceToHost, s.stream), "D2H status");
+			if (sents) { sentOff.resize((size_t)pn + 1); ck(cudaMemcpyAsync(sentOff.data(), retry_.sentOff, ((size_t)pn + 1) * 4, cudaMemcpyDeviceToHost, s.stream), "D2H sentence offsets"); }
 			ck(cudaStreamSynchronize(s.stream), "sync (retry pass)");
 			checkDebug(retry_);
+			if (!tokens) std::fill(tokOff.begin(), tokOff.end(), 0u);
 			const size_t base = out.tokens.size(), nTok = tokOff[pn];
 			out.tokens.resize(base + nTok);
 			if (nTok) ck(cudaMemcpy(out.tokens.data() + base, retry_.packed, nTok * sizeof(DToken), cudaMemcpyDeviceToHost), "D2H tokens");
 			for (uint32_t k = 1; k <= pn; ++k) out.tokOff.push_back((uint32_t)(base + tokOff[k]));
 			out.msTotal += kernelMs(s.ev).total;
 			last.h2dBytes += pT * 2 + ((size_t)pn + 1) * 4; last.d2hBytes += ((size_t)pn * 3 + 1) * 4 + nTok * sizeof(DToken);
+			if (sents)
+			{
+				const float msSents0 = out.msSents;
+				copySents(retry_, s.stream, s.evSents, pn, sentOff.data(), out);
+				out.msTotal += out.msSents - msSents0;
+				last.d2hBytes += ((size_t)pn + 1) * 4;
+			}
 		}
-		if (round + 1 < 2) retryFailed(text, offsets, matchOptions, round + 1, out);
+		if (round + 1 < 2) retryFailed(text, offsets, matchOptions, round + 1, out, outputs);
 	}
 
 	// Gathers the retryable sentences of `out` (the results of the batch text / offsets), in input order, into one contiguous
 	// sub-batch, runs it through retry round `round` and the rounds after it, and puts the results in their places.  Returns how many
 	// sentences it re-ran.
-	size_t Engine::retryFailed(const uint16_t* text, const uint32_t* offsets, uint32_t matchOptions, int round, BatchOutput& out)
+	size_t Engine::retryFailed(const uint16_t* text, const uint32_t* offsets, uint32_t matchOptions, int round, BatchOutput& out, uint32_t outputs)
 	{
 		std::vector<uint32_t> ids;
 		for (uint32_t i = 0; i < (uint32_t)out.status.size(); ++i) if (retryable(out.status[i])) ids.push_back(i);
@@ -562,9 +638,10 @@ namespace kb
 			subOff.push_back((uint32_t)subText.size());
 			sub.status.push_back(out.status[id]);
 		}
-		runRetry(subText.data(), subOff.data(), (uint32_t)ids.size(), matchOptions, round, sub);
-		// splice the retried sentences into the token stream (rare path: rebuild)
-		TokenVec toks; std::vector<uint32_t> tokOff(1, 0);
+		runRetry(subText.data(), subOff.data(), (uint32_t)ids.size(), matchOptions, round, sub, outputs);
+		// splice the retried sentences into the token stream and the sentence ranges (rare path: rebuild)
+		const bool sents = (outputs & OUT_SENTS) != 0;
+		TokenVec toks; std::vector<uint32_t> tokOff(1, 0), sentOff(1, 0), sentBegin, sentEnd;
 		toks.reserve(out.tokens.size() + sub.tokens.size());
 		for (uint32_t i = 0, k = 0; i < (uint32_t)out.status.size(); ++i)
 		{
@@ -574,8 +651,15 @@ namespace kb
 			toks.insert(toks.end(), src.tokens.begin() + src.tokOff[j], src.tokens.begin() + src.tokOff[j + 1]);
 			out.scores[i] = src.scores[j]; out.status[i] = src.status[j];
 			tokOff.push_back((uint32_t)toks.size());
+			if (sents)
+			{
+				sentBegin.insert(sentBegin.end(), src.sentBegin.begin() + src.sentOff[j], src.sentBegin.begin() + src.sentOff[j + 1]);
+				sentEnd.insert(sentEnd.end(), src.sentEnd.begin() + src.sentOff[j], src.sentEnd.begin() + src.sentOff[j + 1]);
+				sentOff.push_back((uint32_t)sentBegin.size());
+			}
 		}
 		out.tokens.swap(toks); out.tokOff.swap(tokOff);
+		if (sents) { out.sentOff.swap(sentOff); out.sentBegin.swap(sentBegin); out.sentEnd.swap(sentEnd); out.msSents += sub.msSents; }
 		out.msTotal += sub.msTotal;
 		return ids.size();
 	}
@@ -593,18 +677,21 @@ namespace kb
 		return v;
 	}
 
-	void Engine::analyze(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, BatchOutput& out)
+	void Engine::analyze(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, BatchOutput& out, uint32_t outputs)
 	{
 		DeviceGuard g{ device };
 		last = Stats{};
+		const bool tokens = (outputs & OUT_TOKENS) != 0;
 		// (the caller may hand in a recycled BatchOutput: keep the vectors' capacity)
 		out.tokOff.assign(1, 0); out.tokens.clear(); out.scores.clear(); out.status.clear();
-		out.msH2D = out.msLattice = out.msViterbi = out.msPack = out.msD2H = out.msTotal = 0;
+		out.sentOff.clear(); out.sentBegin.clear(); out.sentEnd.clear();
+		if (outputs & OUT_SENTS) out.sentOff.push_back(0);
+		out.msH2D = out.msLattice = out.msViterbi = out.msPack = out.msSents = out.msD2H = out.msTotal = 0;
 		if (n == 0) return;
 		if (offsets[0] != 0) throw std::runtime_error("offsets[0] must be 0");
 		for (uint32_t i = 0; i < n; ++i) if (offsets[i + 1] < offsets[i]) throw std::runtime_error("offsets must be non-decreasing");
 		out.tokOff.reserve((size_t)n + 1); out.scores.reserve(n); out.status.reserve(n);
-		out.tokens.reserve(tokenEstimate(offsets[n], n));
+		if (tokens) out.tokens.reserve(tokenEstimate(offsets[n], n));
 		const size_t sentLimit = std::max<size_t>(passSentLimit() / passDivisor(), 1), unitLimit = MAX_UNITS_PER_PASS / passDivisor();
 		const auto fits = [&](size_t units, size_t count) { return units <= unitLimit && count <= sentLimit; };
 		uint32_t i0 = 0, k = 0;
@@ -615,12 +702,12 @@ namespace kb
 				const uint32_t i1 = passEnd(offsets, i0, n, fits);
 				Slot& s = slot_[k & 1];
 				// results are appended in input order: the slot's previous pass (k - 2) is older than the other slot's (k - 1)
-				finishPass(s, out);
-				submitPass(s, text, offsets, i0, i1 - i0, matchOptions, k == 0 ? out.tokens.data() : nullptr);      // (capacity reserved above)
+				finishPass(s, out, outputs);
+				submitPass(s, text, offsets, i0, i1 - i0, matchOptions, k == 0 && tokens ? out.tokens.data() : nullptr, outputs);      // (capacity reserved above)
 				i0 = i1; ++k;
 			}
-			finishPass(slot_[k & 1], out);
-			finishPass(slot_[(k + 1) & 1], out);
+			finishPass(slot_[k & 1], out, outputs);
+			finishPass(slot_[(k + 1) & 1], out, outputs);
 			drainTokenCopies(out);
 		}
 		catch (...)
@@ -628,7 +715,7 @@ namespace kb
 			for (auto& sl : slot_) { if (sl.busy || sl.tokPending) { cudaStreamSynchronize(sl.stream); sl.busy = false; sl.tokPending = false; } }
 			throw;
 		}
-		last.retried = retryFailed(text, offsets, matchOptions, 0, out);
+		last.retried = retryFailed(text, offsets, matchOptions, 0, out, outputs);
 		last.nSentences = n; last.rawUnits = offsets[n]; last.tokens = out.tokens.size();
 		last.msLattice = out.msLattice; last.msViterbi = out.msViterbi; last.msPack = out.msPack;
 	}

@@ -72,13 +72,18 @@ namespace kb
 	};
 	using TokenVec = std::vector<DToken, PinnedNoInitAlloc<DToken>>;
 
+	// what Engine::analyze brings back besides scores and statuses: the token rows, the sentence ranges (Kiwi::splitIntoSents), or both
+	enum : uint32_t { OUT_TOKENS = 1, OUT_SENTS = 2 };
+
 	struct BatchOutput
 	{
-		std::vector<uint32_t> tokOff;      // [n + 1]
+		std::vector<uint32_t> tokOff;      // [n + 1]; all 0 without OUT_TOKENS
 		TokenVec tokens;
 		std::vector<float> scores;
 		std::vector<uint32_t> status;
-		float msH2D = 0, msLattice = 0, msViterbi = 0, msPack = 0, msD2H = 0, msTotal = 0;
+		// OUT_SENTS: the ranges of sentence s are [sentOff[s], sentOff[s + 1]) of sentBegin / sentEnd, UTF-16 units relative to the sentence's text
+		std::vector<uint32_t> sentOff, sentBegin, sentEnd;
+		float msH2D = 0, msLattice = 0, msViterbi = 0, msPack = 0, msSents = 0, msD2H = 0, msTotal = 0;
 	};
 
 	struct Stats
@@ -102,7 +107,8 @@ namespace kb
 		// host buffers in, host buffers out (H2D / D2H inside).  Batches larger than one pass are cut into passes that alternate
 		// between two scratch arenas on two streams: pass k+1's H2D and kernels overlap pass k's tail and D2H.
 		// A sentence that overflows even the escalated retry capacity keeps a non-zero status and an empty token list (no throw).
-		void analyze(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, BatchOutput& out);
+		// `outputs` (OUT_*): OUT_SENTS adds the sentence kernel (sents.cu) after the token emission; without OUT_TOKENS no token row is copied back.
+		void analyze(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, BatchOutput& out, uint32_t outputs = OUT_TOKENS);
 		// AnalyzeOption::blocklist: a patched copy of the candidate table (device memory of this engine's device, Model::blockedCands) replaces
 		// the model's for the calls that follow; nullptr = the model's own table
 		void setCandsOverride(const DCand* deviceTable);
@@ -135,6 +141,9 @@ namespace kb
 			void* cubTemp = nullptr; size_t cubTempBytes = 0;
 			uint16_t* dText = nullptr; uint32_t* dOff = nullptr;
 			uint32_t* lenKeys = nullptr; uint32_t* lenKeysOut = nullptr; uint32_t* idxIn = nullptr; uint32_t* order = nullptr; uint32_t* orderVit = nullptr; void* sortTemp = nullptr; size_t sortTempBytes = 0;
+			// sentence ranges (allocated by the first split): per-sentence counts and their scan [capSent + 1], the packed ranges [capUnits]
+			std::vector<void*> sentBufs; size_t sentCapUnits = 0, sentCapSent = 0;
+			uint32_t* nSents = nullptr; uint32_t* sentOff = nullptr; uint32_t* sentBegin = nullptr; uint32_t* sentEnd = nullptr;
 		};
 		// one in-flight pass: its own scratch arena, stream, events and pinned staging
 		struct Slot
@@ -142,6 +151,7 @@ namespace kb
 			Scratch sc;
 			cudaStream_t stream = nullptr;
 			cudaEvent_t ev[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };      // [6], [7]: around the deferred token copy
+			cudaEvent_t evSents[4] = { nullptr, nullptr, nullptr, nullptr };      // [0], [1]: around the sentence kernels; [2], [3]: around the copy of the ranges
 			uint16_t* hPinText = nullptr; uint32_t* hPinOff = nullptr; size_t pinTextCap = 0, pinOffCap = 0;
 			void* hPinOut = nullptr; size_t pinOutCap = 0;
 			// the pass in flight
@@ -159,16 +169,19 @@ namespace kb
 		void bind(Scratch& sc, const uint16_t* dText, const uint32_t* dOffsets, uint32_t n, uint32_t matchOptions, uint32_t capMul);
 		void uploadConstants();
 		void launchAll(Scratch& sc, cudaStream_t st, cudaEvent_t* ev, uint32_t n);
-		void submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t n, uint32_t matchOptions, DToken* directDst);
+		void ensureSentScratch(Scratch& sc);
+		void launchSents(Scratch& sc, cudaStream_t st, cudaEvent_t* evSents, uint32_t n);
+		void copySents(Scratch& sc, cudaStream_t st, cudaEvent_t* evSents, uint32_t n, const uint32_t* sentOff, BatchOutput& out);
+		void submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t n, uint32_t matchOptions, DToken* directDst, uint32_t outputs);
 		void drainTokenCopies(BatchOutput& out);
 		// SkipBigram states (Knlm node + 8-token history) rarely merge: 8 x the paths per sentence from the start (the first retry round of the
 		// other models), passes 16 x smaller so that the arena stays the same size
 		uint32_t pathScale() const { return model.dev.model_type == 3 ? 8u : 1u; }
 		size_t passDivisor() const { return model.dev.model_type == 3 ? 16 : 1; }
 		size_t pathStride() const { return model.dev.model_type == 3 ? 96 : sizeof(DPath); }      // SkipBigram paths carry their 8-token history (viterbi.cu PathS)
-		void finishPass(Slot& s, BatchOutput& out);
-		void runRetry(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, int round, BatchOutput& out);
-		size_t retryFailed(const uint16_t* text, const uint32_t* offsets, uint32_t matchOptions, int round, BatchOutput& out);
+		void finishPass(Slot& s, BatchOutput& out, uint32_t outputs);
+		void runRetry(const uint16_t* text, const uint32_t* offsets, uint32_t n, uint32_t matchOptions, int round, BatchOutput& out, uint32_t outputs = OUT_TOKENS);
+		size_t retryFailed(const uint16_t* text, const uint32_t* offsets, uint32_t matchOptions, int round, BatchOutput& out, uint32_t outputs);
 		void checkDebug(Scratch& sc);
 	};
 

@@ -68,7 +68,7 @@ namespace kb
 		MF_VOWEL_SHIFT = 28,          // 4 bits CondVowel
 	};
 
-	enum : uint32_t { MM_COMPLEX = 1u, MM_SAISIOT = 2u };
+	enum : uint32_t { MM_COMPLEX = 1u, MM_SAISIOT = 2u, MM_KFORM_YO = 4u };      // MM_KFORM_YO: kform is "요" (the sentence splitter's jx-요 rule)
 	struct alignas(16) DMorph             // 32 B, one vector load
 	{
 		uint32_t feat;

@@ -185,7 +185,7 @@ namespace kb
 			d.feat = feat; d.lm_id = m.lm_morpheme_id; d.combined = m.combined; d.chunk_off = m.chunk_off; d.user_score = m.user_score;
 			d.form_idx = m.form_idx; d.chunk_cnt = m.chunk_cnt; d.combine_socket = m.combine_socket; d.sense_id = m.sense_id;
 			d.nonstd_dialect = m.dialect != 0;
-			d.misc = ((m.flags & KB2_MORPH_COMPLEX) ? MM_COMPLEX : 0) | ((m.flags & KB2_MORPH_SAISIOT) ? MM_SAISIOT : 0);
+			d.misc = ((m.flags & KB2_MORPH_COMPLEX) ? MM_COMPLEX : 0) | ((m.flags & KB2_MORPH_SAISIOT) ? MM_SAISIOT : 0) | (kl == 1 && k0 == 0xC694 ? MM_KFORM_YO : 0);
 			dmorphs[i] = d;
 		}
 
