@@ -31,7 +31,18 @@ extern "C" {
 #define KIWI_MATCH_SERIAL 16
 #define KIWI_MATCH_EMOJI 32
 #define KIWI_MATCH_NORMALIZE_CODA (1 << 16)
+#define KIWI_MATCH_JOIN_NOUN_PREFIX (1 << 17)
+#define KIWI_MATCH_JOIN_NOUN_SUFFIX (1 << 18)
+#define KIWI_MATCH_JOIN_VERB_SUFFIX (1 << 19)
+#define KIWI_MATCH_JOIN_ADJ_SUFFIX (1 << 20)
+#define KIWI_MATCH_JOIN_ADV_SUFFIX (1 << 21)
+#define KIWI_MATCH_SPLIT_COMPLEX (1 << 22)
 #define KIWI_MATCH_Z_CODA (1 << 23)
+#define KIWI_MATCH_COMPATIBLE_JAMO (1 << 24)
+#define KIWI_MATCH_SPLIT_SAISIOT (1 << 25)
+#define KIWI_MATCH_MERGE_SAISIOT (1 << 26)
+#define KIWI_MATCH_JOIN_PARTICLE_YO (1 << 27)
+#define KIWI_MATCH_JOIN_AFFIX (KIWI_MATCH_JOIN_NOUN_PREFIX | KIWI_MATCH_JOIN_NOUN_SUFFIX | KIWI_MATCH_JOIN_VERB_SUFFIX | KIWI_MATCH_JOIN_ADJ_SUFFIX | KIWI_MATCH_JOIN_ADV_SUFFIX)
 #define KIWI_MATCH_ALL (KIWI_MATCH_URL | KIWI_MATCH_EMAIL | KIWI_MATCH_HASHTAG | KIWI_MATCH_MENTION | KIWI_MATCH_SERIAL | KIWI_MATCH_EMOJI | KIWI_MATCH_Z_CODA)
 #define KIWI_MATCH_ALL_WITH_NORMALIZING (KIWI_MATCH_ALL | KIWI_MATCH_NORMALIZE_CODA)
 
@@ -163,8 +174,16 @@ int kiwi_ss_end_position(kiwi_ss_h result, int index);                       /* 
 int kiwi_ss_close(kiwi_ss_h result);                                         /* capi.h:1194 */
 
 /* ---- additive batched interface (flat arrays; what kiwi_analyze_mw drains into) -------------------- */
+/* A token the token-joining options (KIWI_MATCH_JOIN_*, KIWI_MATCH_MERGE_SAISIOT, KIWI_MATCH_JOIN_PARTICLE_YO; joinAffixTokens,
+ * src/Kiwi.cpp:495-588) made of several has no morpheme: its morph_id is KIWI_B200_JOINED_TOKEN | k, where k indexes the batch's
+ * `forms` array (morpheme ids stay far below 2^31).  The entry at forms[k] is
+ *   forms[k], forms[k + 1]   the morpheme id of the token's FIRST component, low 16 bits then high 16 bits (its sense_id and dialect)
+ *   forms[k + 2] ...         the joined form (TokenInfo::str: joinHangul per component, compatibility jamo with KIWI_MATCH_COMPATIBLE_JAMO,
+ *                            coda ㅅ for a merged 사이시옷), terminated by 0.
+ * The row keeps its first component's position, score and flags; its length reaches to the end of its last component. */
+#define KIWI_B200_JOINED_TOKEN 0x80000000u
 typedef struct {
-	uint32_t morph_id;      /* morphToId(PathNode.morph) after unifyMorpheme (PathEvaluator.hpp:1054-1058) */
+	uint32_t morph_id;      /* morphToId(PathNode.morph) after unifyMorpheme (PathEvaluator.hpp:1054-1058), or KIWI_B200_JOINED_TOKEN | k */
 	uint32_t position;      /* original UTF-16 units (Kiwi.cpp:734-737) */
 	float score;            /* PathNode.wordScore */
 	uint16_t length;
@@ -182,6 +201,11 @@ typedef struct {
 	const uint32_t* status;             /* 0 = ok */
 	/* device timing of the last call, milliseconds (CUDA events on the engine's stream) */
 	float ms_h2d, ms_lattice, ms_viterbi, ms_pack, ms_d2h, ms_total;
+	/* the joined tokens' entries (see KIWI_B200_JOINED_TOKEN), forms_size UTF-16 units; NULL when the call had no token-joining option
+	 * (or nothing joined).  KIWI_MATCH_COMPATIBLE_JAMO applies to these forms; forms a caller builds itself from the text or the
+	 * morphemes are the caller's to convert. */
+	const kchar16_t* forms;
+	uint32_t forms_size;
 } kiwi_b200_batch_t;
 
 /* Analyze n sentences given as one UTF-16 blob + offsets[n+1].  Returns NULL and sets kiwi_error() on failure

@@ -20,6 +20,18 @@ LIB_PATH = os.environ.get("KIWI_B200_LIB", os.path.join(_HERE, "libkiwi_b200.so"
 
 MATCH_ALL = 1 | 2 | 4 | 8 | 16 | 32 | (1 << 23)
 MATCH_ALL_WITH_NORMALIZING = MATCH_ALL | (1 << 16)
+# token-joining options (include/kiwi_b200.h KIWI_MATCH_*): joined tokens have morph_id JOINED_TOKEN | k, their form is BatchResult.joined_form
+MATCH_JOIN_NOUN_PREFIX = 1 << 17
+MATCH_JOIN_NOUN_SUFFIX = 1 << 18
+MATCH_JOIN_VERB_SUFFIX = 1 << 19
+MATCH_JOIN_ADJ_SUFFIX = 1 << 20
+MATCH_JOIN_ADV_SUFFIX = 1 << 21
+MATCH_JOIN_AFFIX = MATCH_JOIN_NOUN_PREFIX | MATCH_JOIN_NOUN_SUFFIX | MATCH_JOIN_VERB_SUFFIX | MATCH_JOIN_ADJ_SUFFIX | MATCH_JOIN_ADV_SUFFIX
+MATCH_COMPATIBLE_JAMO = 1 << 24
+MATCH_SPLIT_SAISIOT = 1 << 25
+MATCH_MERGE_SAISIOT = 1 << 26
+MATCH_JOIN_PARTICLE_YO = 1 << 27
+JOINED_TOKEN = 0x80000000
 
 TAG_NAMES = ["UN", "NNG", "NNP", "NNB", "VV", "VA", "MAG", "NR", "NP", "VX", "MM", "MAJ", "IC", "XPN", "XSN", "XSV", "XSA", "XSM", "XR",
              "VCP", "VCN", "SF", "SP", "SS", "SSO", "SSC", "SE", "SO", "SW", "SB", "SL", "SH", "SN", "W_URL", "W_EMAIL", "W_MENTION",
@@ -121,7 +133,7 @@ class Config(C.Structure):
 class _Batch(C.Structure):
     _fields_ = [("n_sentences", C.c_int), ("token_offsets", C.POINTER(C.c_uint32)), ("tokens", C.c_void_p), ("scores", C.POINTER(C.c_float)),
                 ("status", C.POINTER(C.c_uint32)), ("ms_h2d", C.c_float), ("ms_lattice", C.c_float), ("ms_viterbi", C.c_float),
-                ("ms_pack", C.c_float), ("ms_d2h", C.c_float), ("ms_total", C.c_float)]
+                ("ms_pack", C.c_float), ("ms_d2h", C.c_float), ("ms_total", C.c_float), ("forms", C.POINTER(C.c_uint16)), ("forms_size", C.c_uint32)]
 
 
 class _Sents(C.Structure):
@@ -257,9 +269,21 @@ class BatchResult:
     timings_ms: dict
     status: np.ndarray = None      # uint32 [n]: 0 = analysed; non-zero = the sentence exceeded even the escalated device capacity (no tokens)
     _owner: object = None          # the arrays above are views into the library's result buffers (no copy)
+    forms: np.ndarray = None       # uint16: the joined tokens' entries (token-joining options; empty otherwise)
 
     def sentence(self, i: int) -> np.ndarray:
         return self.tokens[self.token_offsets[i]:self.token_offsets[i + 1]]
+
+    def joined_form(self, i: int, k: int):
+        """token k of sentence i made by a token-joining option: (form, morpheme id of its first component); None for any other token"""
+        m = int(self.sentence(i)[k]["morph_id"])
+        if not m & JOINED_TOKEN:
+            return None
+        e = m & ~JOINED_TOKEN
+        end = e + 2
+        while self.forms[end]:
+            end += 1
+        return self.forms[e + 2:end].tobytes().decode("utf-16-le", "surrogatepass"), int(self.forms[e]) | (int(self.forms[e + 1]) << 16)
 
 
 @dataclass
@@ -332,7 +356,8 @@ class Kiwi:
         scores = np.ctypeslib.as_array(b.scores, shape=(n,)) if n else np.zeros(0, np.float32)
         status = np.ctypeslib.as_array(b.status, shape=(n,)) if n else np.zeros(0, np.uint32)
         tm = dict(h2d=b.ms_h2d, lattice=b.ms_lattice, viterbi=b.ms_viterbi, pack=b.ms_pack, d2h=b.ms_d2h, total=b.ms_total)
-        return BatchResult(tok_off, tokens, scores, tm, status, owner)
+        forms = np.ctypeslib.as_array(b.forms, shape=(b.forms_size,)) if b.forms else np.zeros(0, np.uint16)
+        return BatchResult(tok_off, tokens, scores, tm, status, owner, forms)
 
     def analyze_batch(self, texts: Sequence[str], option: AnalyzeOption = None) -> BatchResult:
         blob, offsets = encode_batch(texts)
@@ -347,7 +372,9 @@ class Kiwi:
         r = self.analyze_batch(texts, option)
         out = []
         for i, t in enumerate(texts):
-            toks = [(int(k["morph_id"]), tag_to_string(int(k["tag"])), int(k["position"]), int(k["length"]), float(k["score"])) for k in r.sentence(i)]
+            # (a token made by a token-joining option has no morpheme: -1, as the reference's morphToId(nullptr))
+            toks = [(-1 if int(k["morph_id"]) & JOINED_TOKEN else int(k["morph_id"]), tag_to_string(int(k["tag"])), int(k["position"]), int(k["length"]),
+                     float(k["score"])) for k in r.sentence(i)]
             out.append([(toks, float(r.scores[i]))])
         return out[0] if single else out
 

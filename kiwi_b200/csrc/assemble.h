@@ -8,6 +8,7 @@
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <stdexcept>
 #include <string>
 #include <vector>
 #include "kb_model.h"
@@ -149,5 +150,66 @@ namespace kb
 			AsmTok& t = toks[i];
 			t.wordPosition = st[i].wordPosition; t.sentPosition = st[i].sentPosition; t.lineNumber = st[i].lineNumber; t.subSentPosition = st[i].subSentPosition;
 		}
+	}
+
+	// ---- one sentence's device rows -> the reference's TokenInfo list (insertPathIntoResults src/Kiwi.cpp:714-751, then fillPairedTokenInfo /
+	// fillSentLineInfo, Kiwi.cpp:1149-1154).  The model's host view: morphemes, forms, form characters, character attributes (chr_bmp).
+	struct ResTok { AsmTok a; uint32_t morphId; uint8_t senseId; uint16_t dialect; };
+	inline std::vector<ResTok> assembleRows(const kb2_morph* morphs, const kb2_form* forms, const uint16_t* formChars, const uint32_t* chrBmp,
+		const uint16_t* text, uint32_t rawLen, const DToken* rows, uint32_t n, const uint16_t* joined, size_t joinedSize, uint32_t matchOptions)
+	{
+		// word index of every raw position: getWordPositions, src/Kiwi.cpp:464-485 (a run of spaces ends one word)
+		std::vector<uint16_t> wordPos(rawLen + 1, 0);
+		{
+			uint32_t position = 0; bool continuousSpace = false;
+			for (uint32_t i = 0; i <= rawLen; ++i)
+			{
+				wordPos[i] = (uint16_t)position;
+				if (i < rawLen && attrSpace(chrBmp[text[i]])) { if (!continuousSpace) ++position; continuousSpace = true; }
+				else continuousSpace = false;
+			}
+		}
+		const NormText nt = normalizeWithPosition(text, rawLen, (matchOptions & (1u << 16)) != 0);
+		std::vector<ResTok> out(n);
+		std::vector<AsmTok> at(n);
+		for (uint32_t t = 0; t < n; ++t)
+		{
+			const DToken& d = rows[t];
+			ResTok& r = out[t];
+			AsmTok& a = at[t];
+			a.position = d.position; a.length = d.length; a.tag = d.tag; a.wordPosition = wordPos[d.position];
+			// a joined row (token-joining options) has no morpheme (morphToId(nullptr) = -1); its entry in `joined` holds the first
+			// component's morpheme id (sense id, dialect) and the form the device built (kb_batch.h JOINED_TOKEN)
+			const bool isJoined = (d.morph & JOINED_TOKEN) != 0;
+			const uint32_t entry = d.morph & ~JOINED_TOKEN;
+			if (isJoined && (size_t)entry + 2 >= joinedSize) throw std::runtime_error("joined token without its form");
+			const uint32_t first = isJoined ? (uint32_t)joined[entry] | ((uint32_t)joined[entry + 1] << 16) : d.morph;
+			const kb2_morph& mm = morphs[first];
+			r.morphId = isJoined ? 0xFFFFFFFFu : d.morph;
+			r.senseId = mm.sense_id; r.dialect = mm.dialect;
+			// an OOV noun (own surface form) has no sense (Kiwi.cpp:738-741)
+			if ((d.flags & 1) && ((mm.tag & 0x7F) == T_nng || (mm.tag & 0x7F) == T_nnp)) r.senseId = 0xFF;
+			if (isJoined)
+			{
+				const uint16_t* f = joined + entry + 2;
+				a.form.assign(reinterpret_cast<const char16_t*>(f), std::find(f, joined + joinedSize, (uint16_t)0) - f);
+				continue;      // (never the jx "요" of the sentence rules: Kiwi.cpp:211 tests t.morph)
+			}
+			if (d.flags & 1)
+			{
+				// own substring: two tokens sharing a raw character = that character's syllable body / coda split
+				const bool beginsAtCoda = t > 0 && rows[t - 1].position + rows[t - 1].length > d.position;
+				const bool endsBeforeCoda = t + 1 < n && rows[t + 1].position < d.position + d.length;
+				a.form = ownSubstringForm(nt, d.position, d.length, beginsAtCoda, endsBeforeCoda);
+			}
+			else if (mm.form_idx >= 0) a.form = joinHangulUnits(reinterpret_cast<const char16_t*>(formChars + forms[mm.form_idx].str_off), forms[mm.form_idx].str_len);
+			// Match::compatibleJamo converts every token's form (Kiwi.cpp:726-729); the device converted the joined ones already
+			if (matchOptions & MO_COMPATIBLE_JAMO) for (auto& c : a.form) c = (char16_t)toCompatibleJamo((uint16_t)c);
+			a.kformIsYo = mm.form_idx >= 0 && forms[mm.form_idx].str_len == 1 && formChars[forms[mm.form_idx].str_off] == 0xC694;
+		}
+		fillPaired(at);
+		fillSentLine(at, newlinePositions(text, rawLen));
+		for (uint32_t t = 0; t < n; ++t) out[t].a = std::move(at[t]);
+		return out;
 	}
 }

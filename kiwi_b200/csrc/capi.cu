@@ -167,13 +167,18 @@ static std::string utf16To8(const std::u16string& s)
 // the kernels' option word: the reference's Match bits (include/kiwi/Types.h) + bit 31 = AnalyzeOption::openEnding (no Match flag lives there)
 static uint32_t optionWord(const kiwi_analyze_option_t& o) { return ((uint32_t)o.match_options & 0x7FFFFFFFu) | (o.open_ending ? 0x80000000u : 0u); }
 
-static void checkOption(const kiwi_analyze_option_t& o, int topN, kiwi_pretokenized_h pt)
+// joins: the call honours the token-joining options (join*, mergeSaisiot, joinParticleYo) and compatibleJamo - the analysis calls do; the
+// sentence splitter and the device-resident call refuse them
+static void checkOption(const kiwi_analyze_option_t& o, int topN, kiwi_pretokenized_h pt, bool joins = false)
 {
 	if (topN != 1) throw std::invalid_argument("kiwi_b200 implements the top_n == 1 path only");
 	if (o.allowed_dialects) throw std::invalid_argument("dialects other than standard are outside the kiwi_b200 hot path");
 	if (pt) throw std::invalid_argument("pretokenized spans are outside the kiwi_b200 hot path");
-	const uint32_t unsupported = (3u << 8) | (1u << 17) | (1u << 18) | (1u << 19) | (1u << 20) | (1u << 21) | (1u << 24) | (1u << 26) | (1u << 27) | (1u << 30);
-	if ((uint32_t)o.match_options & unsupported) throw std::invalid_argument("match_options contain a flag outside the kiwi_b200 hot path (oov models, join*, compatibleJamo, mergeSaisiot, useOldSplitter)");
+	const uint32_t joinBits = MO_JOIN_ANY | MO_COMPATIBLE_JAMO;
+	const uint32_t unsupported = (3u << 8) | (1u << 30) | (joins ? 0u : joinBits);
+	if ((uint32_t)o.match_options & unsupported)
+		throw std::invalid_argument(joins ? "match_options contain a flag outside the kiwi_b200 hot path (oov models, useOldSplitter)"
+			: "match_options contain a flag outside the kiwi_b200 hot path (oov models, join*, compatibleJamo, mergeSaisiot, useOldSplitter)");
 }
 
 static kiwi_res* makeRes(kiwi_s* h, const uint16_t* text, uint32_t rawLen, const BatchOutput& bo, uint32_t idx, uint32_t matchOptions)
@@ -181,63 +186,24 @@ static kiwi_res* makeRes(kiwi_s* h, const uint16_t* text, uint32_t rawLen, const
 	auto* r = new kiwi_res;
 	r->score = bo.scores[idx];
 	const Model& m = h->engine->model;
-	// word index of every raw position: getWordPositions, src/Kiwi.cpp:464-485 (a run of spaces ends one word)
-	const uint32_t textLen = rawLen;
-	std::vector<uint16_t> wordPos(textLen + 1, 0);
+	const uint32_t t0 = bo.tokOff[idx], n = bo.tokOff[idx + 1] - t0;
+	std::vector<ResTok> rt = assembleRows(m.hMorphs, m.hForms, m.hFormChars, m.hChrBmp.data(), text, rawLen, bo.tokens.data() + t0, n, bo.forms.data(), bo.forms.size(), matchOptions);
+	r->toks.resize(n);
+	for (uint32_t t = 0; t < n; ++t)
 	{
-		uint32_t position = 0; bool continuousSpace = false;
-		for (uint32_t i = 0; i <= textLen; ++i)
-		{
-			wordPos[i] = (uint16_t)position;
-			if (i < textLen && attrSpace(m.hostChrAttr(text[i]))) { if (!continuousSpace) ++position; continuousSpace = true; }
-			else continuousSpace = false;
-		}
-	}
-	const NormText nt = normalizeWithPosition(text, rawLen, (matchOptions & KIWI_MATCH_NORMALIZE_CODA) != 0);
-	for (uint32_t t = bo.tokOff[idx]; t < bo.tokOff[idx + 1]; ++t)
-	{
-		const DToken& d = bo.tokens[t];
-		kiwi_res::Tok k;
+		const DToken& d = bo.tokens[t0 + t];
+		const AsmTok& a = rt[t].a;
+		kiwi_res::Tok& k = r->toks[t];
 		std::memset(&k.info, 0, sizeof(k.info));
 		k.info.chr_position = d.position; k.info.length = d.length; k.info.tag = d.tag; k.info.score = d.score;
-		k.info.paired_token = (uint32_t)-1;
 		// TokenInfo::typoCost (src/Kiwi.cpp:739) = node cost / tokens of the node (PathEvaluator.hpp:1074), both in the device row's flags
 		k.info.typo_cost = ((d.flags >> 1) & 7) ? (float)((d.flags >> 1) & 7) * 0.5f / (float)((d.flags >> 4) + 1) : 0.f;
-		k.info.word_position = wordPos[d.position];
-		k.morphId = d.morph;
-		const kb2_morph& mm = m.hMorphs[d.morph];
-		k.info.sense_id = mm.sense_id; k.info.dialect = mm.dialect;
-		if (d.flags & 1)
-		{
-			// own substring: two tokens sharing a raw character = that character's syllable body / coda split (assemble.h)
-			const bool beginsAtCoda = t > bo.tokOff[idx] && bo.tokens[t - 1].position + bo.tokens[t - 1].length > d.position;
-			const bool endsBeforeCoda = t + 1 < bo.tokOff[idx + 1] && bo.tokens[t + 1].position < d.position + d.length;
-			k.form = ownSubstringForm(nt, d.position, d.length, beginsAtCoda, endsBeforeCoda);
-			if ((d.tag & 0x7F) == T_nng || (d.tag & 0x7F) == T_nnp) k.info.sense_id = 0xFF;
-		}
-		else if (mm.form_idx >= 0) k.form = joinHangulUnits(reinterpret_cast<const char16_t*>(m.hFormChars + m.hForms[mm.form_idx].str_off), m.hForms[mm.form_idx].str_len);
+		k.info.sense_id = rt[t].senseId; k.info.dialect = rt[t].dialect;
+		k.info.word_position = a.wordPosition; k.info.sent_position = a.sentPosition; k.info.line_number = a.lineNumber;
+		k.info.sub_sent_position = a.subSentPosition; k.info.paired_token = a.pairedToken;
+		k.morphId = rt[t].morphId;
+		k.form = a.form;
 		k.form8 = utf16To8(k.form);
-		r->toks.push_back(std::move(k));
-	}
-	// paired brackets / bullets, sentence / line / sub-sentence numbers, sentence-relative word index
-	// (fillPairedTokenInfo + fillSentLineInfo, src/Kiwi.cpp:1149-1154; restated in assemble.h)
-	{
-		std::vector<AsmTok> at(r->toks.size());
-		for (size_t i = 0; i < at.size(); ++i)
-		{
-			const auto& k = r->toks[i];
-			at[i].position = k.info.chr_position; at[i].length = k.info.length; at[i].tag = k.info.tag; at[i].form = k.form; at[i].wordPosition = k.info.word_position;
-			const kb2_morph& mm = m.hMorphs[k.morphId];
-			at[i].kformIsYo = mm.form_idx >= 0 && m.hForms[mm.form_idx].str_len == 1 && m.hFormChars[m.hForms[mm.form_idx].str_off] == 0xC694;
-		}
-		fillPaired(at);
-		fillSentLine(at, newlinePositions(text, rawLen));
-		for (size_t i = 0; i < at.size(); ++i)
-		{
-			auto& info = r->toks[i].info;
-			info.word_position = at[i].wordPosition; info.sent_position = at[i].sentPosition; info.line_number = at[i].lineNumber;
-			info.sub_sent_position = at[i].subSentPosition; info.paired_token = at[i].pairedToken;
-		}
 	}
 	return r;
 }
@@ -297,6 +263,10 @@ static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offs
 	out.msH2D = out.msLattice = out.msViterbi = out.msPack = out.msSents = out.msD2H = out.msTotal = 0;
 	out.tokens.clear();
 	out.tokOff.assign((size_t)n + 1, 0); out.scores.resize(n); out.status.resize(n);
+	// joined forms: the shards' arrays one after the other; a shard's joined rows move by the forms in front of its own
+	std::vector<uint32_t> formBase(N, 0);
+	out.forms.clear();
+	for (uint32_t r = 0; r < N; ++r) { formBase[r] = (uint32_t)out.forms.size(); out.forms.insert(out.forms.end(), part[r].forms.begin(), part[r].forms.end()); }
 	const bool sents = (outputs & OUT_SENTS) != 0;
 	out.sentOff.assign(sents ? (size_t)n + 1 : 0, 0);
 	for (uint32_t i = 0; i < n; ++i)
@@ -315,6 +285,7 @@ static void analyzeSharded(kiwi_s* h, const uint16_t* text, const uint32_t* offs
 		{
 			const uint32_t cnt = p.tokOff[k + 1] - p.tokOff[k];
 			if (cnt) std::memcpy(out.tokens.data() + out.tokOff[i], p.tokens.data() + p.tokOff[k], (size_t)cnt * sizeof(DToken));
+			if (formBase[r]) for (uint32_t t = out.tokOff[i]; t < out.tokOff[i] + cnt; ++t) if (out.tokens[t].morph & JOINED_TOKEN) out.tokens[t].morph += formBase[r];
 			if (!sents) continue;
 			const uint32_t ns = p.sentOff[k + 1] - p.sentOff[k];
 			std::copy_n(p.sentBegin.data() + p.sentOff[k], ns, out.sentBegin.data() + out.sentOff[i]);
@@ -353,7 +324,7 @@ static int analyzeMulti(kiwi_h handle, ReadFn&& readOne, kiwi_receiver_t receive
 	if (!handle) return KIWIERR_INVALID_HANDLE;
 	try
 	{
-		checkOption(option, top_n, nullptr);
+		checkOption(option, top_n, nullptr, true);
 		const size_t maxBatch = 65536, maxUnits = 16u << 20;
 		int idx = 0, delivered = 0;
 		bool done = false;
@@ -663,7 +634,7 @@ kiwi_res_h kiwi_analyze_w(kiwi_h handle, const kchar16_t* text, int top_n, kiwi_
 	if (!handle) return nullptr;
 	try
 	{
-		checkOption(option, top_n, pretokenized);
+		checkOption(option, top_n, pretokenized, true);
 		uint32_t len = 0;
 		while (text[len]) ++len;
 		const uint32_t off[2] = { 0, len };
@@ -789,7 +760,7 @@ const kiwi_b200_batch_t* kiwi_b200_analyze_batch(kiwi_h handle, const kchar16_t*
 	if (!handle) { setError("invalid handle"); return nullptr; }
 	try
 	{
-		checkOption(option, 1, nullptr);
+		checkOption(option, 1, nullptr, true);
 		if (n < 0) throw std::invalid_argument("n < 0");
 		auto pool = poolOf(handle);
 		BatchHolder* h = nullptr;
@@ -813,6 +784,8 @@ const kiwi_b200_batch_t* kiwi_b200_analyze_batch(kiwi_h handle, const kchar16_t*
 		h->pub.status = h->bo.status.data();
 		h->pub.ms_h2d = h->bo.msH2D; h->pub.ms_lattice = h->bo.msLattice; h->pub.ms_viterbi = h->bo.msViterbi; h->pub.ms_pack = h->bo.msPack;
 		h->pub.ms_d2h = h->bo.msD2H; h->pub.ms_total = h->bo.msTotal;
+		h->pub.forms = (option.match_options & MO_JOIN_ANY) && !h->bo.forms.empty() ? reinterpret_cast<const kchar16_t*>(h->bo.forms.data()) : nullptr;
+		h->pub.forms_size = (uint32_t)h->bo.forms.size();
 		return &h->pub;
 	}
 	catch (const std::exception& e) { setError(e); return nullptr; }

@@ -27,11 +27,14 @@ namespace kb
 		return lo;
 	}
 
-	struct Emitter
+	// JOIN: the token-joining fold runs over every chunk's rows (emit_join_kernel), which needs each row's own surface form: src[i] = the
+	// {own_off, own_len} its pushTok had
+	template<bool JOIN> struct Emitter
 	{
 		const uint16_t* norm; const uint32_t* posTable; uint32_t n, W;
 		DToken* out; uint32_t nTok = 0; uint32_t err = 0;
 		DToken backTok; uint32_t backBegin = 0, backEnd = 0; bool backValid = false, backSkip = false;
+		uint2* src; uint32_t backOwnOff = 0, backOwnLen = 0;
 
 		__device__ Emitter() {}
 
@@ -45,6 +48,7 @@ namespace kb
 				const uint32_t beginPos = upperBound(posTable, n + 1, backBegin) - 1;
 				const uint32_t endPos = lowerBound(posTable, n + 1, backEnd);
 				t.position = beginPos; t.length = (uint16_t)(endPos - beginPos);
+				if constexpr (JOIN) src[nTok] = make_uint2(backOwnOff, backOwnLen);
 				out[nTok++] = t;
 			}
 			backValid = false;
@@ -71,6 +75,7 @@ namespace kb
 			backTok.morph = morph; backTok.tag = (uint8_t)(mm.feat & MF_TAG_MASK); backTok.score = score; backTok.flags = (uint8_t)((ownLen ? 1 : 0) | typoBits);
 			backTok.position = 0; backTok.length = 0;
 			backBegin = begin; backEnd = end; backValid = true; backSkip = false;
+			if constexpr (JOIN) { backOwnOff = ownOff; backOwnLen = ownLen; }
 			if (ownLen)
 			{
 				const uint32_t c0 = ownChar(ownOff, 0);
@@ -92,12 +97,118 @@ namespace kb
 		}
 	};
 
-	__global__ void __launch_bounds__(128) emit_kernel(const BatchView bv, const VitView vv)
+	// ---- token joining (Match::join*, mergeSaisiot, joinParticleYo): joinAffixTokens, /root/reference/src/Kiwi.cpp:495-588 ----------
+	// A joined row keeps its first token's position, score and flags (concatTokens, Kiwi.cpp:487-493), spans to the end of its last one
+	// and carries JOINED_TOKEN | k: its form is not a substring of the text, so it is written to the sentence's form pool at k.
+	struct JoinPool { uint16_t* p = nullptr; uint32_t len = 0, cap = 0; };
+
+	__device__ __forceinline__ bool kformIsYo(uint32_t morph)
 	{
-		const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-		if (s >= bv.n_sent) return;
+		const int32_t fi = c_m.morphs[morph].form_idx;
+		return fi >= 0 && c_m.forms_raw[fi].str_len == 1 && c_m.form_chars[c_m.forms_raw[fi].str_off] == 0xC694;
+	}
+
+	// appends one component's TokenInfo::str (Kiwi.cpp:723-729): joinHangul over its own form (OOV / pattern tokens) or its morpheme's
+	// kform, then, with Match::compatibleJamo, the compatibility jamo.  false: the pool is full.
+	__device__ bool appendForm(JoinPool& jp, const uint16_t* norm, uint32_t morph, uint2 own, bool compat)
+	{
+		const uint16_t* srcChars; uint32_t srcLen;
+		if (own.y) srcChars = (own.x & 0x80000000u) ? c_m.form_chars + c_m.forms_raw[~own.x].str_off : norm + own.x, srcLen = own.y;
+		else
+		{
+			const int32_t fi = c_m.morphs[morph].form_idx;
+			srcChars = fi >= 0 ? c_m.form_chars + c_m.forms_raw[fi].str_off : nullptr; srcLen = fi >= 0 ? c_m.forms_raw[fi].str_len : 0;
+		}
+		const uint32_t start = jp.len;
+		for (uint32_t k = 0; k < srcLen; ++k)
+		{
+			if (jp.len + 4 > jp.cap) return false;      // (3 units at most, and the entry's terminating 0)
+			const uint32_t c = srcChars[k];
+			uint16_t* back = jp.p + jp.len - 1;
+			// joinHangul, include/kiwi/Utils.h:167-205
+			if (jp.len > start && isHangulSyllable(*back) && (*back - 0xAC00u) % 28 == 0)
+			{
+				if (isHangulCoda(c)) { *back = (uint16_t)(*back + (c - 0x11A7)); continue; }
+				if ((0x11A8 <= c && c < 0x1200) || (0xD7CB <= c && c < 0xD800))
+				{
+					const uint32_t onset = (*back - 0xAC00u) / 28 / 21, vowel = (*back - 0xAC00u) / 28 % 21;
+					*back = (uint16_t)(0x1100 + onset);
+					jp.p[jp.len++] = (uint16_t)(0x1161 + vowel);
+				}
+			}
+			jp.p[jp.len++] = (uint16_t)c;
+		}
+		if (compat) for (uint32_t i = start; i < jp.len; ++i) jp.p[i] = toCompatibleJamo(jp.p[i]);
+		return true;
+	}
+
+	// the fold over the rows [c0, nTok), in place and in the reference's rule order.  The reference folds the whole token list again after
+	// each chunk (insertPathIntoResults, Kiwi.cpp:756), which leaves the earlier chunks' rows as they were except the last two: the last row
+	// may join the new chunk's first, and a trailing Z_SIOT may merge into the new chunk's first noun.  So c0 is the start of the chunk's
+	// rows minus two, and a joined row there gets its entry (the pool's last) reopened.
+	__device__ void joinChunk(DToken* out, uint2* src, uint32_t c0, uint32_t& nTok, uint32_t opt, const uint16_t* norm, JoinPool& jp, uint32_t& err)
+	{
+		const uint32_t c1 = nTok;
+		if (c1 < c0 + 2) return;
+		const bool compat = (opt & MO_COMPATIBLE_JAMO) != 0;
+		uint32_t f = c0;
+		DToken cur = out[f];
+		bool joined = false; uint32_t entry = 0;
+		for (uint32_t nx = c0 + 1; nx < c1;)
+		{
+			const DToken nt = out[nx];
+			const uint8_t ct = cur.tag, ntg = nt.tag;
+			const bool curNN = isNNClass(ct), curStem = curNN || ct == T_xr;
+			uint32_t last = nx; uint8_t tag; bool saisiot = false;
+			if ((opt & MO_JOIN_NOUN_PREFIX) && ct == T_xpn && (isNNClass(ntg) || ntg == T_sn)) tag = ntg;
+			else if ((opt & MO_JOIN_NOUN_SUFFIX) && ntg == T_xsn && (curNN || ct == T_sn)) tag = ct;
+			else if ((opt & MO_JOIN_VERB_SUFFIX) && clearIrregular(ntg) == T_xsv && curStem) tag = (uint8_t)(T_vv | (ntg & 0x80));
+			else if ((opt & MO_JOIN_ADJ_SUFFIX) && clearIrregular(ntg) == T_xsa && curStem) tag = (uint8_t)(T_va | (ntg & 0x80));
+			else if ((opt & MO_JOIN_ADV_SUFFIX) && ntg == T_xsm && curStem) tag = T_mag;
+			else if ((opt & MO_MERGE_SAISIOT) && ntg == T_z_siot && curNN && nx + 1 < c1 && isNNClass(out[nx + 1].tag)) { tag = T_nng; last = nx + 1; saisiot = true; }
+			else if ((opt & MO_JOIN_PARTICLE_YO) && ntg == T_jx && kformIsYo(nt.morph) && (ct == T_ec || ct == T_ef)) tag = ct;
+			else
+			{
+				if (joined) jp.p[jp.len++] = 0;
+				out[f++] = cur;
+				cur = nt; src[f] = src[nx];
+				joined = false;
+				++nx;
+				continue;
+			}
+			if (!joined && (cur.morph & JOINED_TOKEN))
+			{
+				// a row an earlier chunk's fold joined: its entry is the last in the pool; drop its terminating 0 and go on appending
+				entry = cur.morph & ~JOINED_TOKEN;
+				if (!jp.len || jp.p[jp.len - 1] != 0) { err = ST_INTERNAL; return; }
+				--jp.len;
+				joined = true;
+			}
+			if (!joined)
+			{
+				// a new entry: the first component's morpheme id, then its form
+				if (jp.len + 3 > jp.cap) { err = ST_TOKEN_OVERFLOW; return; }
+				entry = jp.len;
+				jp.p[jp.len++] = (uint16_t)(cur.morph & 0xFFFF); jp.p[jp.len++] = (uint16_t)(cur.morph >> 16);
+				if (!appendForm(jp, norm, cur.morph, src[f], compat)) { err = ST_TOKEN_OVERFLOW; return; }
+				cur.morph = JOINED_TOKEN | entry;
+				joined = true;
+			}
+			if (saisiot && jp.len > entry + 2) jp.p[jp.len - 1] = (uint16_t)(jp.p[jp.len - 1] + (0x11BA - 0x11A7));      // coda ㅅ on the left form's last unit
+			if (!appendForm(jp, norm, out[last].morph, src[last], compat)) { err = ST_TOKEN_OVERFLOW; return; }
+			cur.tag = tag;
+			cur.length = (uint16_t)(out[last].position + out[last].length - cur.position);
+			nx = last + 1;
+		}
+		if (joined) jp.p[jp.len++] = 0;
+		out[f] = cur;
+		nTok = f + 1;
+	}
+
+	template<bool JOIN> __device__ __forceinline__ void emitSentence(const BatchView& bv, const VitView& vv, uint32_t s)
+	{
 		const int32_t best = vv.best_rec[s];
-		if (best < 0 || bv.status[s]) { vv.n_tokens[s] = 0; return; }
+		if (best < 0 || bv.status[s]) { vv.n_tokens[s] = 0; if constexpr (JOIN) vv.n_forms[s] = 0; return; }
 		const uint32_t t0 = bv.text_off[s], t1 = bv.text_off[s + 1];
 		const uint32_t n = t1 - t0;
 		const uint32_t W = 2 * n + 4;
@@ -112,8 +223,14 @@ namespace kb
 		const DRec* recs = vv.recs + 2 * ((wbase >> 2) + 2 * (size_t)s);
 		const bool splitSaisiot = (bv.match_options >> 25) & 1;
 
-		Emitter e;
+		Emitter<JOIN> e;
 		e.norm = bv.norm + wbase; e.posTable = bv.pos_table + t0 + s; e.n = n; e.W = W; e.out = vv.tokens + wbase;
+		JoinPool jp{};
+		if constexpr (JOIN)
+		{
+			e.src = bv.end_pos_map + wbase;      // (the lattice's end-position map is free once the lattice is built; a join call runs no sentence kernel)
+			jp.p = vv.forms + (size_t)vv.forms_per_unit * wbase; jp.cap = vv.forms_per_unit * W;
+		}
 
 		// record chain, last chunk first
 		uint32_t* chain = bv.ctr + wbase;                // W entries, free after kernel A
@@ -122,6 +239,7 @@ namespace kb
 		uint32_t* steps = bv.ns_to_pos + wbase;          // backtrack scratch (W entries)
 		for (int32_t ci = (int32_t)L - 1; ci >= 0 && !e.err; --ci)
 		{
+			const uint32_t chunkTok0 = e.nTok;
 			const DRec rec = recs[chain[ci]];
 			const DChunk ch = chunks[rec.chunk];
 			const DNode* gnodes = bv.nodes + nbase + ch.node_off;
@@ -187,9 +305,26 @@ namespace kb
 				prevIdx = steps[si];
 			}
 			e.flushBack();
+			if constexpr (JOIN) if (!e.err) joinChunk(e.out, e.src, chunkTok0 > 2 ? chunkTok0 - 2 : 0, e.nTok, bv.match_options, e.norm, jp, e.err);
 		}
 		if (e.err) { bv.status[s] = e.err; vv.n_tokens[s] = 0; vv.score[s] = 0.f; }
 		else vv.n_tokens[s] = e.nTok;
+		if constexpr (JOIN) vv.n_forms[s] = e.err ? 0 : jp.len;
+	}
+
+	__global__ void __launch_bounds__(128) emit_kernel(const BatchView bv, const VitView vv)
+	{
+		const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+		if (s >= bv.n_sent) return;
+		emitSentence<false>(bv, vv, s);
+	}
+
+	// launched instead of emit_kernel when a token-joining match option is set: the same emission, then the fold over every chunk
+	__global__ void __launch_bounds__(128) emit_join_kernel(const BatchView bv, const VitView vv)
+	{
+		const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+		if (s >= bv.n_sent) return;
+		emitSentence<true>(bv, vv, s);
 	}
 
 	cudaError_t set_model_emit(const DevModel& m) { return cudaMemcpyToSymbol(c_m, &m, sizeof(DevModel)); }
@@ -200,10 +335,12 @@ namespace kb
 #ifdef KB_HOSTSIM
 		(void)stream;
 		if (bv.n_sent != 1) return 1;
-		simt::launch(1, 1, [&] { emit_kernel(bv, vv); });      // thread-per-sentence kernel: one lane
+		if (bv.match_options & MO_JOIN_ANY) simt::launch(1, 1, [&] { emit_join_kernel(bv, vv); });      // thread-per-sentence kernel: one lane
+		else simt::launch(1, 1, [&] { emit_kernel(bv, vv); });
 		return cudaSuccess;
 #else
-		emit_kernel<<<(bv.n_sent + 127) / 128, 128, 0, stream>>>(bv, vv);
+		if (bv.match_options & MO_JOIN_ANY) emit_join_kernel<<<(bv.n_sent + 127) / 128, 128, 0, stream>>>(bv, vv);
+		else emit_kernel<<<(bv.n_sent + 127) / 128, 128, 0, stream>>>(bv, vv);
 		return cudaGetLastError();
 #endif
 	}

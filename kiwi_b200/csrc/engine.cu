@@ -108,6 +108,30 @@ namespace kb
 		for (uint32_t i = lane; i < n; i += 32) packed[o + i] = tokens[wbase + i];
 	}
 
+	// token-joining options: the joined forms of every sentence to their place in the packed form array, and the flagged rows' entry offsets
+	// from sentence-relative to array-relative
+	__global__ void join_pack_kernel(uint32_t nSent, const uint32_t* __restrict__ textOff, uint32_t formsPerUnit, const uint16_t* __restrict__ pools,
+		const uint32_t* __restrict__ nForms, const uint32_t* __restrict__ formOff, const uint32_t* __restrict__ nTokens, const uint32_t* __restrict__ tokOff,
+		DToken* __restrict__ packed, uint16_t* __restrict__ packedForms)
+	{
+		const uint32_t lane = threadIdx.x & 31;
+		const uint32_t s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+		if (s >= nSent) return;
+		const size_t fbase = (size_t)formsPerUnit * (2 * (size_t)textOff[s] + 4 * (size_t)s);
+		const uint32_t nf = nForms[s], fo = formOff[s];
+		for (uint32_t i = lane; i < nf; i += 32) packedForms[fo + i] = pools[fbase + i];
+		if (!fo) return;
+		const uint32_t nt = nTokens[s], to = tokOff[s];
+		for (uint32_t i = lane; i < nt; i += 32) if (packed[to + i].morph & JOINED_TOKEN) packed[to + i].morph += fo;
+	}
+
+	// adds `base` to the entry offset of every joined row (the forms of a later pass are appended behind the earlier passes' forms)
+	__global__ void rebase_joined_kernel(uint32_t n, uint32_t base, DToken* __restrict__ rows)
+	{
+		const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+		if (i < n && (rows[i].morph & JOINED_TOKEN)) rows[i].morph += base;
+	}
+
 	// ---- per-device state: one lock and one owner of the kernels' __constant__ model view per CUDA device --------------
 	namespace
 	{
@@ -166,6 +190,7 @@ namespace kb
 		for (void* p : sc.bufs) cudaFree(p);
 		for (void* p : sc.typoBufs) cudaFree(p);
 		for (void* p : sc.sentBufs) cudaFree(p);
+		for (void* p : sc.joinBufs) cudaFree(p);
 		sc = Scratch{};
 	}
 
@@ -265,9 +290,30 @@ namespace kb
 		sc.capUnits = capU; sc.capSent = capB; sc.capText = capT; sc.pathsPerUnit = ppu; sc.pathsConst = pc; sc.nodesPerUnit = npu;
 	}
 
+	// form pool units per normalised-unit slot: a joined form is at most 3 units per unit of its components' sources plus a 3-unit entry frame;
+	// overflow -> ST_TOKEN_OVERFLOW -> retry arena, which carries capMul x the pool like its node capacity
+	static constexpr uint32_t DEFAULT_FORMS_PER_UNIT = 4;
+
+	void Engine::ensureJoinScratch(Scratch& sc, uint32_t perUnit)
+	{
+		if (sc.joinCapUnits < sc.capUnits || sc.joinCapSent < sc.capSent || sc.joinPerUnit != perUnit)
+		{
+			for (void* p : sc.joinBufs) cudaFree(p);
+			sc.joinBufs.clear();
+			auto alloc = [&](size_t bytes) { void* p = nullptr; ck(cudaMalloc(&p, std::max<size_t>(bytes, 256)), "cudaMalloc(join scratch)"); sc.joinBufs.push_back(p); return p; };
+			const size_t units = sc.capUnits * perUnit;
+			sc.vv.forms = (uint16_t*)alloc(units * 2); sc.vv.n_forms = (uint32_t*)alloc((sc.capSent + 1) * 4);
+			sc.formOff = (uint32_t*)alloc((sc.capSent + 1) * 4); sc.packedForms = (uint16_t*)alloc(units * 2);
+			sc.joinCapUnits = sc.capUnits; sc.joinCapSent = sc.capSent; sc.joinPerUnit = perUnit;
+		}
+		sc.vv.forms = (uint16_t*)sc.joinBufs[0]; sc.vv.n_forms = (uint32_t*)sc.joinBufs[1]; sc.vv.forms_per_unit = perUnit;
+	}
+
 	void Engine::bind(Scratch& sc, const uint16_t* dText, const uint32_t* dOffsets, uint32_t n, uint32_t matchOptions, uint32_t capMul)
 	{
 		sc.bv.n_sent = n; sc.bv.text = dText; sc.bv.text_off = dOffsets; sc.bv.match_options = matchOptions;
+		if (matchOptions & MO_JOIN_ANY) ensureJoinScratch(sc, DEFAULT_FORMS_PER_UNIT * capMul);
+		else { sc.vv.forms = nullptr; sc.vv.n_forms = nullptr; sc.vv.forms_per_unit = 0; }
 		sc.bv.typo = TypoView{};
 		if (typo_)
 		{
@@ -334,6 +380,15 @@ namespace kb
 		const uint32_t threads = 256, blocks = (n * 32 + threads - 1) / threads;
 		pack_kernel<<<blocks, threads, 0, st>>>(n, sc.bv.text_off, sc.vv.n_tokens, sc.tokOff, sc.vv.tokens, sc.packed);
 		ck(cudaGetLastError(), "pack_kernel launch");
+		if (sc.bv.match_options & MO_JOIN_ANY)
+		{
+			ck(cudaMemsetAsync(sc.vv.n_forms + n, 0, 4, st), "memset");
+			size_t tb2 = sc.cubTempBytes;
+			ck(cub::DeviceScan::ExclusiveSum(sc.cubTemp, tb2, sc.vv.n_forms, sc.formOff, (int)(n + 1), st), "cub scan");
+			join_pack_kernel<<<blocks, threads, 0, st>>>(n, sc.bv.text_off, sc.vv.forms_per_unit, sc.vv.forms, sc.vv.n_forms, sc.formOff, sc.vv.n_tokens, sc.tokOff, sc.packed, sc.packedForms);
+			ck(cudaGetLastError(), "join_pack_kernel launch");
+			last.kernelLaunches += 2;
+		}
 		ck(cudaEventRecord(ev[4], st), "event");
 		last.kernelLaunches += 6;
 	}
@@ -397,6 +452,17 @@ namespace kb
 		cudaEventElapsedTime(&ms, evSents[0], evSents[1]); out.msSents += ms;
 		cudaEventElapsedTime(&ms, evSents[2], evSents[3]); out.msD2H += ms; out.msTotal += ms;
 		last.d2hBytes += total * 8;
+	}
+
+	// appends the packed forms of a finished launch of n sentences (nForms units, the total of its formOff scan) to `out.forms`, and moves the
+	// entry offsets of its joined rows, out.tokens[tokBegin, end), behind the forms already there
+	void Engine::copyForms(Scratch& sc, uint32_t nForms, size_t tokBegin, BatchOutput& out)
+	{
+		const size_t base = out.forms.size();
+		out.forms.resize(base + nForms);
+		if (nForms) ck(cudaMemcpy(out.forms.data() + base, sc.packedForms, (size_t)nForms * 2, cudaMemcpyDeviceToHost), "D2H joined forms");
+		if (base) for (size_t t = tokBegin; t < out.tokens.size(); ++t) if (out.tokens[t].morph & JOINED_TOKEN) out.tokens[t].morph += (uint32_t)base;
+		last.d2hBytes += (size_t)nForms * 2;
 	}
 
 	// KIWI_B200_SOLO=<blocks>,<warps> (work-queue kernel build): the first <blocks> blocks of the Viterbi wave keep only <warps> warps,
@@ -484,7 +550,8 @@ namespace kb
 		if (sents) ensureSentScratch(s.sc);
 		launchAll(s.sc, s.stream, s.ev, pn);
 		if (sents) launchSents(s.sc, s.stream, s.evSents, pn);
-		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2 + (sents ? (size_t)pn + 1 : 0);
+		const bool join = (matchOptions & MO_JOIN_ANY) != 0;
+		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2 + (sents ? (size_t)pn + 1 : 0) + (join ? 1 : 0);
 		const size_t est = directDst ? std::min(tokenEstimate(pT, pn), (size_t)U) : 0;
 		growPinned(&s.hPinOut, &s.pinOutCap, headWords * 4 + 16);
 		uint32_t* hTokOff = (uint32_t*)s.hPinOut; float* hScore = (float*)(hTokOff + pn + 1); uint32_t* hStatus = (uint32_t*)(hScore + pn); uint32_t* hDbg = hStatus + pn;
@@ -494,6 +561,7 @@ namespace kb
 		ck(cudaMemcpyAsync(hDbg, s.sc.bv.debug, 4, cudaMemcpyDeviceToHost, s.stream), "D2H debug");
 		ck(cudaMemcpyAsync(hDbg + 1, model.dev.debug, 4, cudaMemcpyDeviceToHost, s.stream), "D2H debug");
 		if (sents) ck(cudaMemcpyAsync(hDbg + 2, s.sc.sentOff, ((size_t)pn + 1) * 4, cudaMemcpyDeviceToHost, s.stream), "D2H sentence offsets");
+		if (join) ck(cudaMemcpyAsync(hDbg + 2 + (sents ? pn + 1 : 0), s.sc.formOff + pn, 4, cudaMemcpyDeviceToHost, s.stream), "D2H form total");
 		if (est) ck(cudaMemcpyAsync(directDst, s.sc.packed, est * sizeof(DToken), cudaMemcpyDeviceToHost, s.stream), "D2H tokens");
 		ck(cudaEventRecord(s.ev[5], s.stream), "event");
 		s.busy = true; s.n = pn; s.tokCopied = est;
@@ -526,8 +594,8 @@ namespace kb
 			cudaEventElapsedTime(&ms, s.ev[6], s.ev[7]); out.msD2H += ms; out.msTotal += ms;
 		}
 		const uint32_t pn = s.n;
-		const bool tokens = (outputs & OUT_TOKENS) != 0, sents = (outputs & OUT_SENTS) != 0;
-		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2 + (sents ? (size_t)pn + 1 : 0);
+		const bool tokens = (outputs & OUT_TOKENS) != 0, sents = (outputs & OUT_SENTS) != 0, join = (s.sc.bv.match_options & MO_JOIN_ANY) != 0;
+		const size_t headWords = ((size_t)pn + 1) + 2 * (size_t)pn + 2 + (sents ? (size_t)pn + 1 : 0) + (join ? 1 : 0);
 		const uint32_t* hTokOff = (const uint32_t*)s.hPinOut; const float* hScore = (const float*)(hTokOff + pn + 1); const uint32_t* hStatus = (const uint32_t*)(hScore + pn); const uint32_t* hDbg = hStatus + pn;
 		if (hDbg[0] || hDbg[1]) checkDebug(s.sc);
 		const uint32_t total = tokens ? hTokOff[pn] : 0;
@@ -535,6 +603,21 @@ namespace kb
 		// what the first pass copied on its own is in place already (base == 0 there); make it part of the array before anything can move it
 		const size_t first = std::min<size_t>(total, s.tokCopied);
 		if (first) out.tokens.resize(base + first);
+		const size_t formBase = out.forms.size();
+		if (join && tokens)
+		{
+			// (the rows still to be copied get their entry offsets moved on the device; a pass with a base has no early copy: only the first does)
+			const uint32_t nForms = hDbg[2 + (sents ? pn + 1 : 0)];
+			out.forms.resize(formBase + nForms);
+			if (nForms) ck(cudaMemcpy(out.forms.data() + formBase, s.sc.packedForms, (size_t)nForms * 2, cudaMemcpyDeviceToHost), "D2H joined forms");
+			if (formBase && total)
+			{
+				if (first) throw std::runtime_error("joined forms: a later pass has an early token copy");
+				rebase_joined_kernel<<<(total + 255) / 256, 256, 0, s.stream>>>(total, (uint32_t)formBase, s.sc.packed);
+				ck(cudaGetLastError(), "rebase_joined_kernel launch");
+			}
+			last.d2hBytes += (size_t)nForms * 2;
+		}
 		if (total > first)
 		{
 			if (base + total > out.tokens.capacity()) drainTokenCopies(out);      // the array is about to move
@@ -572,7 +655,7 @@ namespace kb
 		const uint32_t ppu = DEFAULT_PATHS_PER_UNIT * pathScale() * pathMul[round], pc = DEFAULT_PATHS_CONST * pathScale() * pathMul[round], npu = KB_DEFAULT_NODES_PER_UNIT * nodeMul[round];
 		const auto fits = [&](size_t units, size_t count) { return (units * ppu + count * pc) * pathStride() <= budget; };
 		Slot& s = slot_[0];
-		out.tokOff.assign(1, 0); out.tokens.clear(); out.scores.assign(n, 0.f);
+		out.tokOff.assign(1, 0); out.tokens.clear(); out.forms.clear(); out.scores.assign(n, 0.f);
 		if (sents) { out.sentOff.assign(1, 0); out.sentBegin.clear(); out.sentEnd.clear(); }
 		std::vector<uint32_t> subOff, tokOff, sentOff;
 		for (uint32_t i0 = 0, i1; i0 < n; i0 = i1)
@@ -608,6 +691,12 @@ namespace kb
 			const size_t base = out.tokens.size(), nTok = tokOff[pn];
 			out.tokens.resize(base + nTok);
 			if (nTok) ck(cudaMemcpy(out.tokens.data() + base, retry_.packed, nTok * sizeof(DToken), cudaMemcpyDeviceToHost), "D2H tokens");
+			if (tokens && (matchOptions & MO_JOIN_ANY))
+			{
+				uint32_t nForms = 0;
+				ck(cudaMemcpy(&nForms, retry_.formOff + pn, 4, cudaMemcpyDeviceToHost), "D2H form total");
+				copyForms(retry_, nForms, base, out);
+			}
 			for (uint32_t k = 1; k <= pn; ++k) out.tokOff.push_back((uint32_t)(base + tokOff[k]));
 			out.msTotal += kernelMs(s.ev).total;
 			last.h2dBytes += pT * 2 + ((size_t)pn + 1) * 4; last.d2hBytes += ((size_t)pn * 3 + 1) * 4 + nTok * sizeof(DToken);
@@ -642,13 +731,18 @@ namespace kb
 		// splice the retried sentences into the token stream and the sentence ranges (rare path: rebuild)
 		const bool sents = (outputs & OUT_SENTS) != 0;
 		TokenVec toks; std::vector<uint32_t> tokOff(1, 0), sentOff(1, 0), sentBegin, sentEnd;
+		// (the retried sentences' forms go behind the batch's: a sentence that failed has none in `out`)
+		const uint32_t subFormBase = (uint32_t)out.forms.size();
+		out.forms.insert(out.forms.end(), sub.forms.begin(), sub.forms.end());
 		toks.reserve(out.tokens.size() + sub.tokens.size());
 		for (uint32_t i = 0, k = 0; i < (uint32_t)out.status.size(); ++i)
 		{
 			const bool retried = k < ids.size() && ids[k] == i;
 			const BatchOutput& src = retried ? sub : out;
 			const uint32_t j = retried ? k++ : i;
+			const size_t at = toks.size();
 			toks.insert(toks.end(), src.tokens.begin() + src.tokOff[j], src.tokens.begin() + src.tokOff[j + 1]);
+			if (retried && subFormBase) for (size_t t = at; t < toks.size(); ++t) if (toks[t].morph & JOINED_TOKEN) toks[t].morph += subFormBase;
 			out.scores[i] = src.scores[j]; out.status[i] = src.status[j];
 			tokOff.push_back((uint32_t)toks.size());
 			if (sents)
@@ -683,7 +777,7 @@ namespace kb
 		last = Stats{};
 		const bool tokens = (outputs & OUT_TOKENS) != 0;
 		// (the caller may hand in a recycled BatchOutput: keep the vectors' capacity)
-		out.tokOff.assign(1, 0); out.tokens.clear(); out.scores.clear(); out.status.clear();
+		out.tokOff.assign(1, 0); out.tokens.clear(); out.forms.clear(); out.scores.clear(); out.status.clear();
 		out.sentOff.clear(); out.sentBegin.clear(); out.sentEnd.clear();
 		if (outputs & OUT_SENTS) out.sentOff.push_back(0);
 		out.msH2D = out.msLattice = out.msViterbi = out.msPack = out.msSents = out.msD2H = out.msTotal = 0;

@@ -83,6 +83,8 @@ namespace kb
 		std::vector<uint32_t> status;
 		// OUT_SENTS: the ranges of sentence s are [sentOff[s], sentOff[s + 1]) of sentBegin / sentEnd, UTF-16 units relative to the sentence's text
 		std::vector<uint32_t> sentOff, sentBegin, sentEnd;
+		// token-joining options: the joined forms the flagged rows (DToken::morph = JOINED_TOKEN | k) point into; empty otherwise
+		std::vector<uint16_t> forms;
 		float msH2D = 0, msLattice = 0, msViterbi = 0, msPack = 0, msSents = 0, msD2H = 0, msTotal = 0;
 	};
 
@@ -144,6 +146,10 @@ namespace kb
 			// sentence ranges (allocated by the first split): per-sentence counts and their scan [capSent + 1], the packed ranges [capUnits]
 			std::vector<void*> sentBufs; size_t sentCapUnits = 0, sentCapSent = 0;
 			uint32_t* nSents = nullptr; uint32_t* sentOff = nullptr; uint32_t* sentBegin = nullptr; uint32_t* sentEnd = nullptr;
+			// joined forms (allocated by the first call with a token-joining option): the per-sentence pools live in vv.forms; their scan [capSent + 1]
+			// and the packed forms [joinCapUnits]
+			std::vector<void*> joinBufs; size_t joinCapUnits = 0, joinCapSent = 0; uint32_t joinPerUnit = 0;
+			uint32_t* formOff = nullptr; uint16_t* packedForms = nullptr;
 		};
 		// one in-flight pass: its own scratch arena, stream, events and pinned staging
 		struct Slot
@@ -170,6 +176,8 @@ namespace kb
 		void uploadConstants();
 		void launchAll(Scratch& sc, cudaStream_t st, cudaEvent_t* ev, uint32_t n);
 		void ensureSentScratch(Scratch& sc);
+		void ensureJoinScratch(Scratch& sc, uint32_t perUnit);
+		void copyForms(Scratch& sc, uint32_t nForms, size_t tokBegin, BatchOutput& out);
 		void launchSents(Scratch& sc, cudaStream_t st, cudaEvent_t* evSents, uint32_t n);
 		void copySents(Scratch& sc, cudaStream_t st, cudaEvent_t* evSents, uint32_t n, const uint32_t* sentOff, BatchOutput& out);
 		void submitPass(Slot& s, const uint16_t* text, const uint32_t* off, uint32_t i0, uint32_t n, uint32_t matchOptions, DToken* directDst, uint32_t outputs);

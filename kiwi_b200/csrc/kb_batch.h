@@ -85,7 +85,23 @@ namespace kb
 		int32_t* best_rec;           // [n_sent] record of the best stitched result, -1 = none
 		float* score;                // [n_sent]
 		unsigned long long* timing;  // [2 * n_sent] %globaltimer at the start / end of every sentence's Viterbi (diagnostics: the kernel time is its slowest sentence)
+		// token-joining options only (emit_join_kernel): the joined forms of sentence s, forms_per_unit * W_s units at forms_per_unit * wbase
+		// (entry layout: JOINED_TOKEN below); n_forms[s] = units used.  nullptr without a join option.
+		uint16_t* forms;
+		uint32_t* n_forms;           // [n_sent + 1]
+		uint32_t forms_per_unit;
 	};
+
+	// Match bits of the token-joining fold (joinAffixTokens, /root/reference/src/Kiwi.cpp:495-588) and of the form conversion
+	enum : uint32_t
+	{
+		MO_JOIN_NOUN_PREFIX = 1u << 17, MO_JOIN_NOUN_SUFFIX = 1u << 18, MO_JOIN_VERB_SUFFIX = 1u << 19, MO_JOIN_ADJ_SUFFIX = 1u << 20,
+		MO_JOIN_ADV_SUFFIX = 1u << 21, MO_COMPATIBLE_JAMO = 1u << 24, MO_MERGE_SAISIOT = 1u << 26, MO_JOIN_PARTICLE_YO = 1u << 27,
+		MO_JOIN_ANY = MO_JOIN_NOUN_PREFIX | MO_JOIN_NOUN_SUFFIX | MO_JOIN_VERB_SUFFIX | MO_JOIN_ADJ_SUFFIX | MO_JOIN_ADV_SUFFIX | MO_MERGE_SAISIOT | MO_JOIN_PARTICLE_YO,
+	};
+	// DToken::morph of a joined token: JOINED_TOKEN | k, k = offset of its entry in the forms array.  An entry is the first component's
+	// morpheme id (low 16 bits, high 16 bits) followed by the joined form and a terminating 0 (include/kiwi_b200.h KIWI_B200_JOINED_TOKEN).
+	constexpr uint32_t JOINED_TOKEN = 0x80000000u;
 
 	enum : uint32_t { ST_OK = 0, ST_NODE_OVERFLOW = 1, ST_CHUNK_OVERFLOW = 2, ST_PATH_OVERFLOW = 3, ST_TOKEN_OVERFLOW = 4, ST_TOO_LONG = 5, ST_INTERNAL = 6, ST_TYPO_OVERFLOW = 7 };
 

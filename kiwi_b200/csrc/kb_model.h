@@ -46,6 +46,24 @@ namespace kb
 	KB_HD bool isHangulSyllable(uint32_t c) { return 0xAC00 <= c && c < 0xD7A4; }
 	KB_HD bool isHangulCoda(uint32_t c) { return 0x11A8 <= c && c < 0x11A8 + 27; }
 	KB_HD bool isHighSurrogate(uint32_t c) { return (c & 0xFC00) == 0xD800; }
+	// Match::compatibleJamo: a conjoining consonant becomes its Hangul Compatibility Jamo (U+3131-314E, the 30 consonants ㄱ..ㅎ in
+	// Unicode order).  The 19 choseong U+1100-1112 are the compatibility consonants without the 11 clusters ㄳ ㄵ ㄶ ㄺ-ㅀ ㅄ; the 27
+	// jongseong U+11A8-11C2 are the compatibility consonants without the 3 that never close a syllable, ㄸ ㅃ ㅉ.  Others: unchanged.
+	KB_HD uint32_t nthSetBit(uint32_t mask, uint32_t n)
+	{
+		uint32_t j = 0;
+		for (;; ++j) if ((mask >> j) & 1) { if (!n) break; --n; }
+		return j;
+	}
+	KB_HD uint16_t toCompatibleJamo(uint16_t c)
+	{
+		constexpr uint32_t all = (1u << 30) - 1;
+		constexpr uint32_t onsets = all & ~((1u << 2) | (1u << 4) | (1u << 5) | (0x7Fu << 9) | (1u << 19));
+		constexpr uint32_t codas = all & ~((1u << 7) | (1u << 18) | (1u << 24));
+		if (0x1100 <= c && c < 0x1113) return (uint16_t)(0x3131 + nthSetBit(onsets, c - 0x1100u));
+		if (0x11A8 <= c && c < 0x11C3) return (uint16_t)(0x3131 + nthSetBit(codas, c - 0x11A8u));
+		return c;
+	}
 	KB_HD uint32_t mergeSurrogate(uint32_t h, uint32_t l) { return (((h & 0x3FF) << 10) | (l & 0x3FF)) + 0x10000; }
 
 	// ---- morpheme feature word (DMorph::feat)
